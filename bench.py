@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — end-to-end images/sec of the SEED-X hot path on N B200s of one node (one process per GPU, replicas).
+"""bench.py — end-to-end images/sec of the SEED-X hot path on N GPUs of one node (one process per GPU, replicas).
 
 Workloads (BASELINE.json `configs`; `--workload`):
   i2i (default, the headline metric: 448x448 in -> 1024x1024 out; configs[2] = its de-tokenizer stage at batch 4)
@@ -16,8 +16,8 @@ Workloads (BASELINE.json `configs`; `--workload`):
 Weights: random-init at the full architecture sizes (no checkpoints offline).  Ranks are independent replicas (weak scaling), NCCL only
 gathers the finished images.
 
-Prints ONE JSON line (rank 0).  `value` = device-resident inputs; `e2e` = pinned-host inputs copied in and results copied out inside the
-timed region.  `roofline` is for the dominant launch, the CUDA-graphed UNet sample-forward (6.75 TFLOP per sample, SURVEY.md A.4).
+Prints ONE JSON line (rank 0).  `value` = the --steps timed steps, device-resident inputs; `e2e` = one further probe step with pinned-host
+inputs copied in and results copied out inside its timed region.  `roofline` is for the dominant launch, the CUDA-graphed UNet sample-forward (6.75 TFLOP per sample, SURVEY.md A.4).
 `cpu_baseline` / `--impl reference`: the CPU oracle (oracle/, the reference's PyTorch path restated) timed on the host cores, ONE UNIT PER
 STAGE (a ViT view, LLaMA layers in prefill and in decode, a UNet sample-forward, a VAE decode / encode) and extrapolated to the workload by
 the exact number of units the unmodified reference would execute (BASELINE.md §4); the per-stage CPU seconds are printed.
@@ -82,12 +82,11 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d["bf16_tflops_sustained"], d["hbm_gbs"], "measured (MEASURED_PEAKS.json, sustained bf16 cuBLAS)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md: ~1.4 PFLOP/s sustained, 6.65 TB/s)"
+    return 989.0, 3350.0, "fallback (H100 SXM data sheet at 700 W: 989 TFLOP/s dense fp16, 3.35 TB/s HBM3)"
 
 
 def measured_traffic():
-    """per-launch DRAM bytes from the committed ncu captures (profiles/r02_traffic.json, written by tools/summarize_traffic.py from the raw
-    ncu CSVs next to it); None when no capture is committed for this batch size"""
+    """per-launch DRAM bytes of a traffic capture stored as profiles/r02_traffic.json; empty when none is present"""
     p = os.path.join(ROOT, "profiles", "r02_traffic.json")
     return json.load(open(p)) if os.path.exists(p) else {}
 
@@ -332,6 +331,29 @@ def run_reference(args):
 # ------------------------------------------------------------------------------------------------------------------------------------------
 # comprehension workload (auxiliary line)
 # ------------------------------------------------------------------------------------------------------------------------------------------
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Write each array as out_dir/<name>.npy in float32, in its own shape.  When the arrays exceed DUMP_LIMIT_BYTES together, every array
+    above 1 MB is cut to a fixed, seeded sample of its flat elements (the same positions from run to run) and written as <name>_sample.npy,
+    so that two builds can be compared element for element."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    arrs = {k: torch.as_tensor(v).detach().cpu().to(torch.float32) for k, v in arrays.items()}
+    small = {k for k, t in arrs.items() if 4 * t.numel() <= (1 << 20)}       # always written whole
+    big_total = sum(4 * t.numel() for k, t in arrs.items() if k not in small)
+    budget = DUMP_LIMIT_BYTES - 4096 * len(arrs) - sum(4 * arrs[k].numel() for k in small)   # room for the .npy headers
+    for k, t in arrs.items():
+        if k not in small and big_total > budget:
+            keep = max(1, t.numel() * budget // big_total)
+            idx = torch.randperm(t.numel(), generator=torch.Generator().manual_seed(0))[:keep].sort().values
+            t = t.reshape(-1)[idx]
+            k = k + "_sample"
+        np.save(os.path.join(out_dir, k + ".npy"), t.numpy())
+
+
 def run_comprehension(args, eng, rank, world, peaks_, cpu_base):
     """--workload comprehension = BASELINE.json configs[1]: 1 x 448^2 image (any-res 1x1 -> 2 ViT views) + 32-token prompt -> 128 greedy text tokens,
     batch 1 per GPU (EOS suppressed so every step decodes exactly 128 tokens).  Auxiliary line: tokens/s, ms per token, decode HBM roofline."""
@@ -347,6 +369,8 @@ def run_comprehension(args, eng, rank, world, peaks_, cpu_base):
     ids, mask = eng.build_prompt(2, text_ids, force_image=False)
     P = int(ids.numel())
 
+    last_out = {}
+
     def step(e2e):
         v = views_host.cuda(non_blocking=True) if e2e else views_dev
         feats = eng.vit(v)
@@ -356,23 +380,26 @@ def run_comprehension(args, eng, rank, world, peaks_, cpu_base):
         out = eng.agent.generate_batch(eng.tok, [req], max_new_tokens=new_tok, suppress_eos=True)[0]   # reads the ids back to the host (d2h)
         return out
 
-    def timed(e2e):
+    def timed(e2e, n):
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         n0 = _lib.launch_count()
         e0.record()
-        for _ in range(args.steps):
+        for _ in range(n):
             out = step(e2e)
         e1.record()
         torch.cuda.synchronize()
         assert len(out["ids"]) == new_tok
+        last_out["ids"] = torch.as_tensor(out["ids"])
         return sdist.max_over_ranks(e0.elapsed_time(e1), "cuda"), _lib.launch_count() - n0
 
     for _ in range(args.warmup):
         step(False)
     with ClockSampler(int(os.environ.get("LOCAL_RANK", "0"))) as cs:
-        ms_dev, launches = timed(False)
-        ms_e2e, _ = timed(True)
+        ms_dev, launches = timed(False, args.steps)          # the timed steps
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, last_out)
+        ms_e2e, _ = timed(True, 1)                            # one end-to-end probe step (host copies included)
     trace.enable(True)
     trace.mark("start")
     step(False)
@@ -387,10 +414,10 @@ def run_comprehension(args, eng, rank, world, peaks_, cpu_base):
             "unit": "tokens/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_dev / args.steps, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f16", "data": "synthetic",
             "config": {"workload": "seedx_comprehension_448 (BASELINE.json configs[1]): prompt %d tokens incl. 2 x 64 image rows, 128 new tokens, EOS suppressed" % P,
-                       "weights": "random-init, full sizes", "l2": "26 GB of weights per token step exceed the 126 MB L2"},
+                       "weights": "random-init, full sizes", "l2": "26 GB of weights per token step exceed the 50 MB L2"},
             "stage_detail_ms": detail,
-            "e2e": {"value": toks / (ms_e2e / 1e3), "unit": "tokens/s", "h2d_bytes_per_step": views_host.numel() * 4 + P * 8,
-                    "d2h_bytes_per_step": (P + new_tok) * 4, "ms_per_step": ms_e2e / args.steps},
+            "e2e": {"value": world * new_tok / (ms_e2e / 1e3), "unit": "tokens/s", "h2d_bytes_per_step": views_host.numel() * 4 + P * 8,
+                    "d2h_bytes_per_step": (P + new_tok) * 4, "ms_per_step": ms_e2e, "steps": 1},
             "gpu_launches": launches, "clocks": cs.summary(),
             "roofline": {"bound": "hbm", "kernel": "CUDA-graph replay of one decode step (gemv_mma_kernel = 84 % of it)", "achieved": gb / (dec_ms / 1e3) if dec_ms else None,
                          "peak": hbm_peak, "unit": "GB/s", "frac": gb / (dec_ms / 1e3) / hbm_peak if dec_ms else None,
@@ -410,6 +437,8 @@ def main():
     ap.add_argument("--denoise-steps", type=int, default=50)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--small", action="store_true", help="debug: tiny models (NOT a valid benchmark)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned as DIR/<name>.npy (float32, <= 64 MB in all)")
     ap.add_argument("--workload", default="i2i", choices=sorted(WORKLOADS),
                     help="i2i (default, the headline metric) | edit (configs[3]) | anyres (configs[4]) | comprehension (configs[1], tokens/s)")
     args = ap.parse_args()
@@ -493,13 +522,18 @@ def main():
     if W["text_tokens"]:
         d2h_bytes += B * W["text_tokens"] * 4
     gather_buf = None
+    last_out = {}
+    # initial latents of every step: one seeded draw, rounded through fp16 as the pipeline's randn_tensor does, so that the inputs are the same
+    # in every run (the global CUDA generator's state depends on everything that drew from it before)
+    noise = synth.randn(f"bench_latents_rank{rank}", (B, 4, 128, 128)).half().float().cuda()
 
     def step(e2e):
         v = views_host.cuda(non_blocking=True) if e2e else views_dev
         src = None
         if wl == "edit":
             src = src_host.cuda(non_blocking=True) if e2e else src_dev
-        u8 = eng.generate(v, patch_pos, text_ids, steps=args.denoise_steps, n_views=n_views, source_images=src, text_tokens=W["text_tokens"])
+        u8 = eng.generate(v, patch_pos, text_ids, steps=args.denoise_steps, noise=noise, n_views=n_views, source_images=src,
+                          text_tokens=W["text_tokens"])
         nonlocal gather_buf
         if world > 1:                                  # the only collective: gather finished images on every rank (NCCL / NVLink)
             gather_buf = sdist.gather_images(u8, gather_buf)
@@ -521,17 +555,18 @@ def main():
             log(f"warmup {i}: {eng.stage_ms()}")
     sync()
 
-    def timed(e2e):
+    def timed(e2e, n):
         sync()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         n0 = _lib.launch_count()
         stages = []
         e0.record()
-        for _ in range(args.steps):
-            step(e2e)
+        for _ in range(n):
+            u8 = step(e2e)
             stages.append(eng._events)
         e1.record()
         sync()
+        last_out["images"] = u8.clone()
         ms = sdist.max_over_ranks(e0.elapsed_time(e1), "cuda")
         st = {k: statistics.mean(a.elapsed_time(b) for (a, b) in [(ev[i], ev[i + 1]) for ev in stages])
               for i, k in enumerate(("vit_ms", "llm_ms", "detok_ms"))}
@@ -539,12 +574,14 @@ def main():
 
     if rank == 0:       # one nvidia-smi poller per job (8 of them would only add host noise); rank 0's GPU stands for the box
         with ClockSampler(local) as cs:
-            ms_dev, launches, stages = timed(e2e=False)
-            ms_e2e, _, _ = timed(e2e=True)
+            ms_dev, launches, stages = timed(False, args.steps)     # the timed steps
+            if args.dump_outputs:
+                dump_outputs(args.dump_outputs, last_out)
+            ms_e2e, _, _ = timed(True, 1)                           # one end-to-end probe step (host copies included)
         clocks = cs.summary()
     else:
-        ms_dev, launches, stages = timed(e2e=False)
-        ms_e2e, _, _ = timed(e2e=True)
+        ms_dev, launches, stages = timed(False, args.steps)
+        ms_e2e, _, _ = timed(True, 1)
         clocks = None
     # one extra untimed step with section marks on (seedx_b200.trace): where the step goes, stage by stage
     from seedx_b200 import trace
@@ -566,14 +603,15 @@ def main():
         eng.llm.generate_greedy_batch(p_ids, p_emb, img_ids=None, max_new_tokens=65, eos_id=None, suppress_eos=True)
         decode_step_ms = trace.summary().get("llm.decode", 0.0) / 64
     trace.enable(False)
-    # transparency: the same timed loop with jump-forward off (every forced image token takes its own decode step, as in the reference)
+    # transparency: one probe step with jump-forward off (every forced image token takes its own decode step, as in the reference), after one
+    # untimed step that captures that mode's decode graph
     token_loop = None
     if world == 1 and not args.small and eng.llm.jump_forward and wl == "i2i":
         try:
             eng.llm.jump_forward = False
             step(e2e=False)
-            ms_tl, _, st_tl = timed(e2e=False)
-            token_loop = {"value": B * args.steps / (ms_tl / 1e3), "unit": "images/s", "ms_per_step": ms_tl / args.steps, "stage_ms_per_step": st_tl,
+            ms_tl, _, st_tl = timed(False, 1)
+            token_loop = {"value": B / (ms_tl / 1e3), "unit": "images/s", "ms_per_step": ms_tl, "steps": 1, "stage_ms_per_step": st_tl,
                           "note": "SEEDX_JUMP_FORWARD=0 behaviour: the 65 forced image tokens decoded one step at a time"}
         except Exception as exc:                          # never let the extra measurement take the headline down
             token_loop = {"error": repr(exc)}
@@ -583,7 +621,7 @@ def main():
     if rank == 0:
         imgs = world * B * args.steps
         value = imgs / (ms_dev / 1e3)
-        e2e_v = imgs / (ms_e2e / 1e3)
+        e2e_v = world * B / (ms_e2e / 1e3)
         traffic = measured_traffic()
         # dominant launch: the CUDA-graphed UNet sample-forward (branches x B samples per launch, 50 launches per step), timed live here with
         # CUDA events on the launching stream
@@ -599,9 +637,9 @@ def main():
         unet_ms = e0.elapsed_time(e1) / reps
         n_samples = branches * B
         achieved = UNET_TFLOP * n_samples / (unet_ms / 1e3) if not args.small else None
-        # the dominant kernel's dominant shape, timed alone with CUDA events on the launching stream: gemm_tc_kernel<256,2> on the GEGLU
+        # the dominant kernel's dominant shape, timed alone with CUDA events on the launching stream: gemm_tc_kernel on the GEGLU
         # projection of the UNet feed-forward (60 launches per forward = 16 % of it, the largest single line of the launch list); three
-        # operand sets (393 MB) rotate so that no launch finds its inputs in the 126 MB L2
+        # operand sets (393 MB) rotate so that no launch finds its inputs in the 50 MB L2
         dom = None
         if not args.small:
             from seedx_b200 import ops
@@ -622,7 +660,7 @@ def main():
             us = e0.elapsed_time(e1) * 1e3 / n_l
             fl = 2.0 * Mg * Ng * Kg
             tkey = f"geglu_gemm_M{Mg}_bytes"
-            dom = {"kernel": "gemm_tc_kernel<256,2> (tcgen05 cta_group::2), GEGLU projection M=%d N=%d K=%d, bias + GELU gating fused" % (Mg, Ng, Kg),
+            dom = {"kernel": "gemm_tc_kernel (wgmma), GEGLU projection M=%d N=%d K=%d, bias + GELU gating fused" % (Mg, Ng, Kg),
                    "launch_us": us, "achieved": fl / us / 1e6, "unit": "TFLOP/s", "peak": tensor_peak, "frac": fl / us / 1e6 / tensor_peak,
                    "algorithmic_bytes": 2 * (Mg * Kg + Ng * Kg + Mg * Ng // 2), "traffic": traffic.get(tkey),
                    "traffic_source": traffic.get("source") if traffic.get(tkey) is not None else None}
@@ -685,12 +723,11 @@ def main():
             "stage_roofline": stage_roof,
             "without_jump_forward": token_loop,
             "e2e": {"value": e2e_v, "unit": "images/s", "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": d2h_bytes,
-                    "ms_per_step": ms_e2e / args.steps},
+                    "ms_per_step": ms_e2e, "steps": 1},
             "gpu_launches": launches,
             "clocks": clocks,
             "roofline": {"bound": "tensor",
-                         "kernel": "CUDA-graph launch of one UNet sample-forward (%d samples): gemm_tc_kernel (GEMM + implicit-GEMM conv) and tcgen05 attention, "
-                                   "per-kernel shares and DRAM bytes in profiles/r02_unet_forward_launches_*.csv / .md" % n_samples,
+                         "kernel": "CUDA-graph launch of one UNet sample-forward (%d samples): gemm_tc_kernel (GEMM + implicit-GEMM conv) and wgmma attention" % n_samples,
                          "achieved": achieved, "peak": tensor_peak, "unit": "TFLOP/s", "frac": (achieved / tensor_peak) if achieved else None,
                          "dominant_kernel": dom, "traffic": traffic.get(f"unet_forward_{n_samples}samples_bytes"),
                          "traffic_source": traffic.get("source") if traffic.get(f"unet_forward_{n_samples}samples_bytes") is not None else None,

@@ -1,5 +1,5 @@
 /*
- * seedx.h — C ABI of libseedx.so, the B200 (sm_100a) kernel library behind the SEED-X inference hot path.
+ * seedx.h — C ABI of libseedx.so, the H100 (sm_90a) kernel library behind the SEED-X inference hot path.
  *
  * The reference (AILab-CVC/SEED-X) has no FFI/plugin layer: every FLOP is reached through
  * torch.nn.functional / xformers / diffusers library calls made from its nn.Module.forward methods.
@@ -40,7 +40,7 @@ int64_t seedx_launch_count(void);
 int seedx_set_pdl(int on);
 
 /* ------------------------------------------------------------------------------------------------
- * Tensor-core GEMM / implicit-GEMM convolution (tcgen05 + TMEM accumulators + TMA operand staging)
+ * Tensor-core GEMM / implicit-GEMM convolution (wgmma, register accumulators, TMA operand staging)
  *
  *   D[b][m][n] = epilogue( alpha * sum_k A[b][m][k] * B[b][n][k] )         A, B fp16, fp32 accumulate
  *
@@ -109,13 +109,14 @@ typedef struct seedx_gemm_args {
 } seedx_gemm_args;
 
 int seedx_gemm_f16(const seedx_gemm_args* args, void* stream);
-/* A/B switch for the CTA-pair variant (tcgen05 cta_group::2: one 256 x tile_n accumulator tile over two SMs, each CTA staging its own
- * 128 rows of A and half of the B tile): 0 = off, 1 = auto (default), 2 = whenever legal */
+/* A/B switch for the cluster-pair variant (two CTAs on vertically adjacent 128 x tile_n tiles, each CTA loading its own 128 rows of A and
+ * half of the B tile, which TMA multicasts to both): 0 = off, 1 = auto (default; single-CTA tiles, the faster choice measured on H100),
+ * 2 = whenever legal */
 void seedx_gemm_set_cluster(int mode);
 /* developer aid: device buffer of 8 uint64 per CTA that receives %globaltimer phase stamps of the following GEMM launches (NULL = off) */
 void seedx_gemm_set_debug(void* device_buffer);
-/* Stream-K schedule for launches whose last wave of whole tiles would leave SMs idle (e.g. M = 8192, N = 1280: 192 pair-tiles on 74 CTA pairs =
- * 2.6 waves): every cluster takes an equal share of the (tile, k-block) iterations; partial accumulators of split tiles go through a workspace.
+/* Stream-K schedule of the cluster-pair kernels (seedx_gemm_set_cluster(2)) for launches whose last wave of whole tiles would leave SMs idle (e.g. M = 8192, N = 1280: 192 pair-tiles on 66 cluster pairs =
+ * 2.9 waves): every cluster takes an equal share of the (tile, k-block) iterations; partial accumulators of split tiles go through a workspace.
  * seedx_gemm_set_workspace hands the library that workspace (>= 32 MB recommended, 256-byte aligned, first 16 KB zero-filled by the caller, owned
  * by the caller, used by one stream at a time); without it, or with mode 0, every launch is data-parallel.  mode: 0 off, 1 auto (default), 2 always. */
 int seedx_gemm_set_workspace(void* device_buffer, int64_t bytes);
@@ -144,10 +145,9 @@ typedef struct seedx_attn_args {
 } seedx_attn_args;
 
 int seedx_attention_f16(const seedx_attn_args* args, void* stream);
-/* implementation switch for A/B tests: 0 = auto (two-query-tile tcgen05/TMEM kernel when d <= 128 and sq >= 256, one-tile tcgen05
- * kernel when sq >= 128, else mma.sync), 1 = always mma.sync, 2 = never the two-tile kernel */
+/* implementation switch for A/B tests: 0 = auto (wgmma kernel when d <= 128, sq >= 64 and sk >= 16, else mma.sync), 1 = always mma.sync */
 void seedx_attention_set_impl(int impl);
-int seedx_attention_last_impl(void); /* most recent call: 3 = tcgen05 two-tile, 2 = tcgen05 one-tile, 1 = mma.sync */
+int seedx_attention_last_impl(void); /* most recent call: 2 = wgmma, 1 = mma.sync */
 
 /* ------------------------------------------------------------------------------------------------
  * LayerNorm (rms=0) / RMSNorm (rms=1) over the last dimension, fp32 statistics.

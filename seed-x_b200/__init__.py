@@ -1,2 +1,2 @@
-"""seedx-b200: B200-native (sm_100a) inference kernels + host for the SEED-X ViT -> LLaMA -> SDXL pipeline."""
+"""seedx-b200: H100-native (sm_90a) inference kernels + host for the SEED-X ViT -> LLaMA -> SDXL pipeline."""
 from ._version import __version__  # noqa: F401

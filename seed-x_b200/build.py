@@ -1,4 +1,4 @@
-"""Build libseedx.so (all CUDA sources under csrc/) for sm_100a with nvcc, in-tree.
+"""Build libseedx.so (all CUDA sources under csrc/) for sm_90a with nvcc, in-tree.
 
 Object files are cached per source under seed-x_b200/lib/obj and rebuilt when the source (or a header) is newer.
 """
@@ -13,7 +13,7 @@ LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(LIBDIR, "obj")
 LIB = os.path.join(LIBDIR, "libseedx.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "--use_fast_math" if False else "-DSEEDX_NO_FAST_MATH"]
 
 
@@ -47,7 +47,7 @@ def build(verbose=False, force=False):
         with ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(run, jobs))
     if jobs or not os.path.exists(LIB):
-        run([NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a"])
+        run([NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a"])
     return LIB
 
 

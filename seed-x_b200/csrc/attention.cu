@@ -3,8 +3,8 @@
 //   O[b,h,i,:] = softmax_j( scale * Q[b,h,i,:] . K[b,h,j,:]  (+ causal mask) ) V[b,h,j,:]
 //
 // fp16 operands, fp32 scores / statistics / accumulation.  One CTA = 64 query rows x one (batch, head); 4 warps,
-// 16 rows each; K/V tiles of 64 keys double-buffered through cp.async.  Tensor-core path of this revision is
-// mma.sync.m16n8k16 (HMMA); the tcgen05/TMEM variant is the planned replacement (DESIGN.md "next").
+// 16 rows each; K/V tiles of 64 keys double-buffered through cp.async, mma.sync.m16n8k16.  The wgmma kernel
+// (attention_wg.cu) takes every problem it is built for; this one covers the rest (head dim > 128, fewer than 64 queries).
 //
 // Replaces: src/models/tokenizer/qwen_visual.py:204-215 (ViT MHSA, d=104), :136-146 (nn.MultiheadAttention of the
 // Resampler, d=128/160), src/models/mllm/modeling_llama_xformer.py:225-237 (xformers memory_efficient_attention,
@@ -274,10 +274,9 @@ static int launch_attn(const AttnParams& p, int B, int H, cudaStream_t st) {
 }  // namespace seedx
 
 namespace seedx {
-int attention_tc_try(const seedx_attn_args* a, cudaStream_t st);
-int attention_pp_try(const seedx_attn_args* a, cudaStream_t st);
-static int g_attn_impl = 0;  // 0 = auto (two-tile tcgen05 kernel, else one-tile tcgen05 kernel, else mma.sync), 1 = force mma.sync, 2 = skip the two-tile kernel
-static int g_attn_last = 0;  // implementation used by the most recent call: 3 = tcgen05 two-tile, 2 = tcgen05 one-tile, 1 = mma.sync
+int attention_wg_try(const seedx_attn_args* a, cudaStream_t st);
+static int g_attn_impl = 0;  // 0 = auto (wgmma kernel when eligible, else mma.sync), 1 = force mma.sync
+static int g_attn_last = 0;  // implementation used by the most recent call: 2 = wgmma, 1 = mma.sync
 }
 using namespace seedx;
 
@@ -305,15 +304,8 @@ extern "C" int seedx_attention_f16(const seedx_attn_args* a, void* stream) {
   p.scale_log2 = a->scale * 1.4426950408889634f;
   p.causal = a->causal;
   cudaStream_t st = (cudaStream_t)stream;
-  if (g_attn_impl == 0) {
-    const int rc = attention_pp_try(a, st);
-    if (rc >= 0) {
-      g_attn_last = 3;
-      return rc;
-    }
-  }
-  if (g_attn_impl == 0 || g_attn_impl == 2) {
-    const int rc = attention_tc_try(a, st);
+  if (g_attn_impl != 1) {
+    const int rc = attention_wg_try(a, st);
     if (rc >= 0) {
       g_attn_last = 2;
       return rc;

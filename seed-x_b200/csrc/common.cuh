@@ -1,5 +1,5 @@
-// seedx-b200: shared device helpers (sm_100a only).
-// Raw PTX wrappers for mbarrier / TMA / tcgen05 + small math utilities.
+// seedx-b200: shared device helpers (sm_90a).
+// Raw PTX wrappers for mbarrier / TMA / clusters + small math utilities (warpgroup MMA: wgmma.cuh).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -18,7 +18,7 @@ int check_cuda(cudaError_t e, const char* what);
 
 // ---- programmatic dependent launch (PDL).  Every kernel of this library is launched through launch_k() with the
 // programmatic-stream-serialization attribute and begins its data-dependent part with pdl_wait(): a kernel's launch latency and
-// prologue (barrier init, TMEM allocation, descriptor prefetch, weight prefetch) then overlap the tail of its predecessor, in
+// prologue (barrier init, descriptor prefetch, weight prefetch) then overlap the tail of its predecessor, in
 // eager streams and inside captured CUDA graphs alike.  seedx_set_pdl(0) (or SEEDX_PDL=0) turns the attribute off.
 int pdl_enabled();
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;\n" ::: "memory"); }
@@ -122,38 +122,6 @@ SEEDX_DEVINL void tma_load_4d(uint32_t dst, const void* tmap, uint32_t bar, int 
       : "memory");
 }
 
-// ----------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
-// ----------------------------------------------------------------------------------------------
-SEEDX_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-SEEDX_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
-
-template <uint32_t kCols>
-SEEDX_DEVINL void tmem_alloc(uint32_t smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_dst), "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-template <uint32_t kCols>
-SEEDX_DEVINL void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "n"(kCols) : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc], fp16/bf16 operands, one CTA
-SEEDX_DEVINL void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// make all previously issued MMAs arrive on an mbarrier when they retire
-SEEDX_DEVINL void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar)
-               : "memory");
-}
-
-
 
 // ---- TMA stores (shared -> global), bulk async groups, proxy fence ---------------------------------
 SEEDX_DEVINL void tma_store_3d(const void* tmap, uint32_t src, int c0, int c1, int c2) {
@@ -194,142 +162,31 @@ SEEDX_DEVINL uint32_t mapa_cluster(uint32_t saddr, uint32_t rank) {
 SEEDX_DEVINL void mbar_arrive_cluster(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];\n" ::"r"(cluster_addr) : "memory");
 }
-// ---- CTA pair (cta_group::2): both CTAs issue their own TMA loads, all transaction bytes land on the LEADER's mbarrier
-SEEDX_DEVINL void tma_load_3d_2sm(uint32_t dst, const void* tmap, uint32_t leader_bar, int c0, int c1, int c2) {
+// TMA load delivered to the same shared-memory offset of every CTA in `mask`; each destination's mbarrier at `bar` receives its bytes
+SEEDX_DEVINL void tma_load_3d_mc(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2, uint16_t mask) {
   asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];\n" ::
-          "r"(dst),
-      "l"(tmap), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-SEEDX_DEVINL void tma_load_4d_2sm(uint32_t dst, const void* tmap, uint32_t leader_bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
-      "[%2];\n" ::"r"(dst),
-      "l"(tmap), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-template <uint32_t kCols>
-SEEDX_DEVINL void tmem_alloc_2sm(uint32_t smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_dst), "n"(kCols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;\n" ::: "memory");
-}
-template <uint32_t kCols>
-SEEDX_DEVINL void tmem_dealloc_2sm(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "n"(kCols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A (128 rows from each CTA's smem) * B (N/2 rows from each CTA's smem): M = 256 over the SM pair
-SEEDX_DEVINL void umma_f16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// commit of the pair's MMAs arriving on the mbarrier at the same offset in both CTAs
-SEEDX_DEVINL void umma_commit_2sm(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n" ::"r"(bar),
-               "h"((uint16_t)3)
-               : "memory");
-}
-
-// K-major operand tile, 128-byte swizzle, rows of 64 fp16 (=128 B); 8-row groups are 1024 B apart.
-SEEDX_DEVINL uint64_t umma_desc_k_sw128(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);  // start address
-  d |= (uint64_t)1 << 16;                    // LBO (ignored for swizzled K-major)
-  d |= (uint64_t)(1024 >> 4) << 32;          // SBO
-  d |= (uint64_t)1 << 46;                    // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                    // SWIZZLE_128B
-  return d;
-}
-// instruction descriptor: fp16 x fp16 -> fp32, both K-major, M x N tile
-SEEDX_DEVINL constexpr uint32_t umma_idesc_f16(int M, int N) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// 32 lanes x 32 columns of fp32 accumulators -> 32 registers per thread (thread = TMEM lane)
-SEEDX_DEVINL void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5}], [%2], %6;\n" ::"r"(dst),
+      "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "h"(mask)
       : "memory");
 }
 
-// D[tmem] (+)= A[tmem] * B[smem desc]  (A operand read from tensor memory: fp16 pairs packed per 32-bit column)
-SEEDX_DEVINL void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// MN-major operand tile (e.g. V[keys][d] used as B = V^T): 128-byte swizzle, 64-element (128 B) rows along MN, rows of the K
-// dimension 128 B apart, 8-row groups 1024 B apart (SBO), successive 64-element MN chunks `lbo_bytes` apart (LBO).
-SEEDX_DEVINL uint64_t umma_desc_mn_sw128(uint32_t saddr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// 32 lanes x 32 columns store (registers -> TMEM), thread = lane
-SEEDX_DEVINL void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]),
-      "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]),
-      "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-SEEDX_DEVINL void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]),
-      "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-SEEDX_DEVINL void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-// N = 16 or 32 consecutive 32-bit columns of this thread's TMEM lane
+// ---- register budget of warp-specialised kernels (warpgroup-wide)
 template <int N>
-SEEDX_DEVINL void tmem_ld_n(uint32_t taddr, uint32_t (&r)[N]) {
-  static_assert(N == 16 || N == 32, "tmem_ld_n: 16 or 32 columns");
-  if constexpr (N == 16) tmem_ld16(taddr, r);
-  else tmem_ld32(taddr, r);
+SEEDX_DEVINL void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(N));
 }
 template <int N>
-SEEDX_DEVINL void tmem_st_n(uint32_t taddr, const uint32_t (&r)[N]) {
-  static_assert(N == 16 || N == 32, "tmem_st_n: 16 or 32 columns");
-  if constexpr (N == 16) tmem_st16(taddr, r);
-  else tmem_st32(taddr, r);
+SEEDX_DEVINL void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(N));
 }
-SEEDX_DEVINL void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory"); }
+// named barrier over `threads` threads (warp multiples)
+SEEDX_DEVINL void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(threads) : "memory"); }
 SEEDX_DEVINL float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;\n" : "=f"(y) : "f"(x));
   return y;
 }
 
-SEEDX_DEVINL void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------
 // math

@@ -1,11 +1,11 @@
-// seedx-b200: tcgen05 tensor-core GEMM / implicit-GEMM convolution for sm_100a.
+// seedx-b200: wgmma tensor-core GEMM / implicit-GEMM convolution for sm_90a.
 //
-//   D[b][m][n] = epi( alpha * sum_k A[b][m][k] * B[b][n][k] )      fp16 operands, fp32 accumulate in TMEM
+//   D[b][m][n] = epi( alpha * sum_k A[b][m][k] * B[b][n][k] )      fp16 operands, fp32 accumulate in registers
 //
-// Persistent, warp-specialised: warp 0 = TMA producer, warp 1 = MMA issuer (+TMEM owner), warps 2..5 = epilogue.
+// Persistent, warp-specialised: warpgroup 0 = TMA producer, warpgroups 1 and 2 = wgmma on 64 rows each of the 128-row tile, then the epilogue.
 // Operands are staged by TMA into 128B-swizzled K-major tiles (BM=128 x BK=64, BN x BK=64) through a
-// STAGES-deep mbarrier ring; the accumulator is double-buffered in TMEM (2 x BN columns) so the epilogue of
-// tile i overlaps the main loop of tile i+1.  In conv mode the A tile of k-step (tap, channel-chunk) is a
+// STAGES-deep mbarrier ring; the producer keeps filling it with the next tile's k-blocks while the consumers run
+// the epilogue of the current one.  In conv mode the A tile of k-step (tap, channel-chunk) is a
 // shifted [th x tw] pixel window of the NHWC image fetched by a 4-D tensor map, out-of-bounds = zero padding
 // (im2col-free implicit GEMM).
 //
@@ -14,6 +14,7 @@
 #include <cstdlib>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 #include "../../include/seedx.h"
 
 namespace seedx {
@@ -63,32 +64,33 @@ constexpr int BM = 128;
 constexpr int BK = 64;
 constexpr int A_STAGE_BYTES = BM * BK * 2;
 
-constexpr int EPI_WARPS = 8;                       // two warps per TMEM lane quarter, alternating 32-column chunks
-constexpr int GEMM_THREADS = 64 + EPI_WARPS * 32;  // warp 0 = TMA, warp 1 = MMA, warps 2..9 = epilogue
+constexpr int EPI_WARPS = 8;                       // the two consumer warpgroups: 64 accumulator rows each, then the epilogue of those rows
+constexpr int GEMM_THREADS = 128 + EPI_WARPS * 32; // warpgroup 0 = TMA producer (one thread), warpgroups 1, 2 = MMA + epilogue
 constexpr int SMEM_LIMIT = 227 * 1024;
 constexpr int EPI_OUT_BYTES = 4096;                      // per epilogue warp: output tiles (2 x <=2 KB, or 1 x 4 KB)
 constexpr int EPI_RES_BYTES = 8192;                      // per epilogue warp: residual tiles, ideally every chunk of a 256-wide tile in flight
 constexpr int MAX_STAGES = 8;
 constexpr int VEC_BYTES = 1024;                          // one per-tile column vector of the epilogue (bias_n | LayerNorm column sums), 256 fp32
-
-constexpr int pow2_cols(int c) { return c <= 32 ? 32 : c <= 64 ? 64 : c <= 128 ? 128 : c <= 256 ? 256 : 512; }
+// The epilogue works on rows of 32 accumulator columns (lane = row).  The accumulators live in the wgmma fragment layout (a thread holds 2 rows x
+// 2 columns of every 8-column group), so each warpgroup passes 64 columns at a time through shared memory: 64 rows x ACC_LD fp32.
+// ACC_LD = 72: the fragment's 8-byte stores hit 32 distinct banks per half warp.
+constexpr int ACC_LD = 72;
+constexpr int ACC_WG_BYTES = 64 * ACC_LD * 4;
+constexpr int ACC_STAGE_BYTES = 2 * ACC_WG_BYTES;
 
 template <int BN, int CL = 1>
 struct TileCfg {
-  static_assert(BN % 16 == 0 && BN >= 32 && BN <= 256, "UMMA N for M=128/256: multiple of 16, <= 256");
-  static constexpr int B_STAGE_BYTES = (BN / CL) * BK * 2;   // a CTA of a pair stages only its half of the B tile
+  static_assert(BN % 16 == 0 && BN >= 32 && BN <= 256, "wgmma N: multiple of 16, <= 256");
+  static constexpr int B_STAGE_BYTES = BN * BK * 2;   // in a cluster pair each CTA loads half of it and multicasts that half to both
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
   // pipeline depth for a given amount of epilogue staging (runtime: depends on whether a residual is streamed through shared memory)
   // `tail_bytes` = barriers (512) + the per-tile epilogue vectors (1 KB per vector in use).  The dynamic shared memory is declared 1024-byte
-  // aligned (the 128-byte-swizzled tiles need it), so no alignment slack is budgeted: every kilobyte decides whether one more pipeline stage fits
-  // (a 2 KB vector region that cost the 256-wide residual tiles their fourth stage made every short-K GEMM ~10 % slower).
+  // aligned (the 128-byte-swizzled tiles need it), so no alignment slack is budgeted.
   static int stages_for(int epi_bytes, int tail_bytes) {
-    const int fit = (SMEM_LIMIT - tail_bytes - epi_bytes) / STAGE_BYTES;
+    const int fit = (SMEM_LIMIT - tail_bytes - epi_bytes - ACC_STAGE_BYTES) / STAGE_BYTES;
     return fit > MAX_STAGES ? MAX_STAGES : fit;
   }
-  static int smem_for(int stages, int epi_bytes, int tail_bytes) { return stages * STAGE_BYTES + epi_bytes + tail_bytes; }
-  // two accumulator stages; the last 32-column epilogue chunk of a stage may over-read up to 16 columns -> keep them allocated
-  static constexpr int TMEM_COLS = pow2_cols(2 * BN + 16);
+  static int smem_for(int stages, int epi_bytes, int tail_bytes) { return stages * STAGE_BYTES + ACC_STAGE_BYTES + epi_bytes + tail_bytes; }
 };
 
 SEEDX_DEVINL unsigned long long gtime_ns() {
@@ -106,8 +108,7 @@ SEEDX_DEVINL float apply_act(float x, int act) {
 
 // Work list of one cluster: segments (tile, k-blocks [kb0, kb1)).  Data-parallel: whole tiles first, first + step, ...  Stream-K: the
 // iterations [it, it1) of the linearised (tile, k-block) space, cut at tile boundaries.
-// SK is a compile-time property of the kernel: with the schedule as a run-time flag the data-parallel launches (the large majority) ran ~10 %
-// slower than round 1's kernel — measured with tools/ab_gemm2.py — although none of the stream-K code executed.
+// SK is a compile-time property of the kernel, so that the data-parallel launches (the large majority) carry none of the stream-K code.
 struct SegState {
   long long it, it1;
   int t_next;
@@ -137,12 +138,10 @@ SEEDX_DEVINL bool seg_next(const GemmParams& p, SegState& s, int n_clusters, int
   return true;
 }
 
-// CL = CTAs per MMA (1, or 2 = a CTA pair on one 256 x BN tile, tcgen05 cta_group::2).  In pair mode each CTA stages its own 128 rows
-// of A and only HALF of the B tile (BN/2 rows); the leader CTA (cluster rank 0) issues tcgen05.mma.cta_group::2, which reads both
-// CTAs' shared memory and writes both CTAs' tensor memory (128 accumulator rows each).  Operand bytes an SM has to ingest per FLOP
-// drop by a third, which is what bounds the single-CTA kernel (measured: TMA multicast of B does NOT help, cta_group::2 does).
-// All TMA transaction bytes of the pair complete on the leader's `full` barrier; the leader's commits arrive on both CTAs' `empty`
-// and `tmem_full` barriers; both CTAs' epilogue warps arrive on the leader's `tmem_empty` barrier.
+// CL = CTAs per cluster (1, or 2 = two CTAs on vertically adjacent 128 x BN tiles of the same column block).  In a pair each CTA loads its own
+// 128 rows of A and HALF of the B tile, which TMA multicasts into both CTAs' shared memory: each SM fetches a quarter fewer operand bytes from L2.
+// A stage of a CTA is refilled only when the consumers of BOTH CTAs have released it (the peer writes into it), so every consumer warpgroup
+// arrives on the `empty` barriers of both CTAs.
 template <int BN, int CL, bool SK>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmD,
@@ -153,15 +152,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   const uint32_t smem_base = smem_u32(smem_raw);
   if ((smem_base & 1023u) != 0u) __trap();                          // the launch budgets no alignment slack (TileCfg::smem_for)
-  const uint32_t epi_base = smem_base + STAGES * Cfg::STAGE_BYTES;  // 1024-aligned
+  const uint32_t acc_base = smem_base + STAGES * Cfg::STAGE_BYTES;  // accumulator hand-over, ACC_WG_BYTES per consumer warpgroup
+  const uint32_t epi_base = acc_base + ACC_STAGE_BYTES;             // 1024-aligned
   const uint32_t bar_base = epi_base + (uint32_t)(EPI_WARPS * p.epi_warp_bytes);
-  // barrier layout (8 B each): full[STAGES], empty[STAGES], tmem_full[2], tmem_empty[2], then tmem ptr
+  // barrier layout (8 B each): full[STAGES], empty[STAGES], residual[EPI_WARPS][4]
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * STAGES + 2 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-  auto res_bar = [&](int w, int i) { return bar_base + 8u * (2 * STAGES + 6 + 4 * w + i); };  // residual tile landed (per epilogue warp, <= 4 buffers)
+  auto res_bar = [&](int w, int i) { return bar_base + 8u * (2 * STAGES + 4 * w + i); };  // residual tile landed (per epilogue warp, <= 4 buffers)
   const uint32_t vec_base = bar_base + 512u;       // [bias_n tile | colsum tile], 256 fp32 each: staged once per tile, read as broadcast 128-bit loads
 
   const int warp = threadIdx.x >> 5;
@@ -173,67 +170,54 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), EPI_WARPS * CL);  // pair mode: the leader's barrier collects both CTAs' epilogue warps
+      mbar_init(empty_bar(s), 2 * CL);  // one arrival per consumer warpgroup of every CTA that reads this CTA's B half
     }
     for (int w = 0; w < EPI_WARPS; ++w)
       for (int i = 0; i < 4; ++i) mbar_init(res_bar(w, i), 1);
     mbar_fence_init();
   }
-  if (warp == 1) {
-    if (CL == 1) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-    else tmem_alloc_2sm<Cfg::TMEM_COLS>(tmem_slot);   // the same warp id in both CTAs of the pair
-  }
-  tc_fence_before();
   __syncthreads();
-  if (CL > 1) cluster_sync_all();  // peer barriers are initialised before any remote arrive / transaction can reach them
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];\n" : "=r"(tmem_base) : "r"(tmem_slot));
-  // everything above touched only this CTA's shared/tensor memory: under programmatic dependent launch it ran while the previous
-  // kernel was still draining.  Operands, residual and output may be that kernel's data: wait for it here.
+  if (CL > 1) cluster_sync_all();  // peer barriers are initialised before any remote arrive / multicast transaction can reach them
   if (threadIdx.x == 0) GEMM_STAMP(1);
   // tile space: (batch, n block, m group) with CL consecutive m blocks per group; a cluster walks groups, CTA `crank` takes m = group*CL + crank
   const int m_groups = (p.m_blocks + CL - 1) / CL;
   const int tiles_per_batch = m_groups * p.n_blocks;
   const int num_tiles = tiles_per_batch * p.batch;
   const int tile0 = (int)blockIdx.x / CL, tile_step = (int)gridDim.x / CL;
-  // Weights never depend on the kernel before this one: the B halves of the first stages of this CTA's first tile are requested BEFORE the
-  // dependency wait (their bytes are already counted on the `full` barriers; the A halves follow after the wait).
+  // B half of a stage: rows [n_blk*BN + crank*BN/CL, +BN/CL), at the same offset in every CTA of the cluster
+  auto load_b = [&](uint32_t sb, uint32_t bar, int kb, int n_blk, int b) {
+    if (CL == 1) tma_load_3d(sb, &tmB, bar, kb * BK, n_blk * BN, p.b_batched ? b : 0);
+    else tma_load_3d_mc(sb + (uint32_t)(crank * (BN / CL) * BK * 2), &tmB, bar, kb * BK, n_blk * BN + crank * (BN / CL), p.b_batched ? b : 0,
+                        (uint16_t)((1u << CL) - 1u));
+  };
+  // Weights never depend on the kernel before this one: the B tiles of the first stages of this CTA's first tile are requested BEFORE the
+  // dependency wait (their bytes are already counted on the `full` barriers; the A tiles follow after the wait).
   int b_pre = 0;
   {
     SegState s0 = seg_init<SK>(p, tile0, tile_step, num_tiles);
     int t, kb0, kb1;
-#ifndef SEEDX_GEMM_NO_BPRE
     if (p.b_static && seg_next<SK>(p, s0, tile_step, num_tiles, t, kb0, kb1)) {
       b_pre = (kb1 - kb0) < STAGES ? (kb1 - kb0) : STAGES;
       if (warp == 0 && lane == 0) {
         const int b = t / tiles_per_batch;
         const int n_blk = (t - b * tiles_per_batch) / m_groups;
         for (int i = 0; i < b_pre; ++i) {
-          const uint32_t sb = smem_base + i * Cfg::STAGE_BYTES + A_STAGE_BYTES;
-          if (CL == 1) {
-            mbar_expect_tx(full_bar(i), Cfg::STAGE_BYTES);
-            tma_load_3d(sb, &tmB, full_bar(i), (kb0 + i) * BK, n_blk * BN, p.b_batched ? b : 0);
-          } else {
-            if (crank == 0) mbar_expect_tx(full_bar(i), CL * Cfg::STAGE_BYTES);
-            tma_load_3d_2sm(sb, &tmB, mapa_cluster(full_bar(i), 0), (kb0 + i) * BK, n_blk * BN + crank * (BN / CL), p.b_batched ? b : 0);
-          }
+          mbar_expect_tx(full_bar(i), Cfg::STAGE_BYTES);
+          load_b(smem_base + i * Cfg::STAGE_BYTES + A_STAGE_BYTES, full_bar(i), kb0 + i, n_blk, b);
         }
       }
     }
-#endif
   }
+  // everything above touched only this CTA's shared memory (and weights): under programmatic dependent launch it ran while the previous
+  // kernel was still draining.  Operands, residual and output may be that kernel's data: wait for it here.
   pdl_wait();
   pdl_trigger();
   if (threadIdx.x == 0) GEMM_STAMP(2);
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ------------------------------------------------ TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       SegState ss = seg_init<SK>(p, tile0, tile_step, num_tiles);
@@ -260,95 +244,53 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           mbar_wait(empty_bar(stage), phase ^ 1u);
           const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
           const uint32_t sb = sa + A_STAGE_BYTES;
-          const bool b_done = first_seg && (kb - kb0 < b_pre);   // this stage's barrier is armed and its B half is in flight already
-          if (CL == 1) {
-            if (!b_done) mbar_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
-            if (p.conv) {
-              const int tap = kb / p.c_chunks;
-              const int cc = kb - tap * p.c_chunks;
-              const int kh = tap / p.taps_w;
-              const int kw = tap - kh * p.taps_w;
-              tma_load_4d(sa, &tmA, full_bar(stage), cc * BK, w0 + kw - p.pad, h0 + kh - p.pad, img);
-            } else {
-              tma_load_3d(sa, &tmA, full_bar(stage), kb * BK, m_blk * BM, b);
-            }
-            if (!b_done) tma_load_3d(sb, &tmB, full_bar(stage), kb * BK, n_blk * BN, p.b_batched ? b : 0);
+          const bool b_done = first_seg && (kb - kb0 < b_pre);   // this stage's barrier is armed and its B tile is in flight already
+          if (!b_done) mbar_expect_tx(full_bar(stage), Cfg::STAGE_BYTES);
+          if (p.conv) {
+            const int tap = kb / p.c_chunks;
+            const int cc = kb - tap * p.c_chunks;
+            const int kh = tap / p.taps_w;
+            const int kw = tap - kh * p.taps_w;
+            tma_load_4d(sa, &tmA, full_bar(stage), cc * BK, w0 + kw - p.pad, h0 + kh - p.pad, img);
           } else {
-            // pair mode: the leader arms its barrier for the bytes of BOTH CTAs; every load names the leader's barrier
-            const uint32_t lbar = mapa_cluster(full_bar(stage), 0);
-            if (crank == 0 && !b_done) mbar_expect_tx(full_bar(stage), CL * Cfg::STAGE_BYTES);
-            if (p.conv) {
-              const int tap = kb / p.c_chunks;
-              const int cc = kb - tap * p.c_chunks;
-              const int kh = tap / p.taps_w;
-              const int kw = tap - kh * p.taps_w;
-              tma_load_4d_2sm(sa, &tmA, lbar, cc * BK, w0 + kw - p.pad, h0 + kh - p.pad, img);
-            } else {
-              tma_load_3d_2sm(sa, &tmA, lbar, kb * BK, m_blk * BM, b);
-            }
-            if (!b_done) tma_load_3d_2sm(sb, &tmB, lbar, kb * BK, n_blk * BN + crank * (BN / CL), p.b_batched ? b : 0);   // my half of the B tile
+            tma_load_3d(sa, &tmA, full_bar(stage), kb * BK, m_blk * BM, b);
           }
+          if (!b_done) load_b(sb, full_bar(stage), kb, n_blk, b);
           if (++stage == STAGES) {
             stage = 0;
             phase ^= 1u;
           }
         }
-        first_seg = false;
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------ MMA issuer (single thread; pair mode: the leader CTA only)
-    if (lane == 0 && crank == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(BM * CL, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      SegState ss = seg_init<SK>(p, tile0, tile_step, num_tiles);
-      int t, kb0, kb1;
-      bool first_seg = true;
-      while (seg_next<SK>(p, ss, tile_step, num_tiles, t, kb0, kb1)) {
-        mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          if (first_seg && kb == kb0) GEMM_STAMP(3);
-          tc_fence_after();
-          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES;
-          const uint64_t adesc = umma_desc_k_sw128(sa);
-          const uint64_t bdesc = umma_desc_k_sw128(sa + A_STAGE_BYTES);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            // advance 16 fp16 = 32 B inside the 128B swizzle atom: +2 in the (addr >> 4) field
-            if (CL == 1) umma_f16(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, ((kb - kb0) | k) != 0);
-            else umma_f16_2sm(d_tmem, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, ((kb - kb0) | k) != 0);
-          }
-          if (CL == 1) umma_commit(empty_bar(stage));  // smem slot reusable once these MMAs retire
-          else umma_commit_2sm(empty_bar(stage));      // ... in both CTAs
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        if (CL == 1) umma_commit(tfull_bar(acc));  // accumulator complete
-        else umma_commit_2sm(tfull_bar(acc));
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1u;
         first_seg = false;
       }
     }
   } else {
-    // ------------------------------------------------ epilogue warps (TMEM -> regs -> global)
-    const int lane_grp = warp & 3;            // TMEM lanes [32*lane_grp, +32) are accessible to this warp
-    const int chunk0 = ((warp - 2) >> 2) * 32;  // warps 2..5 take even 32-column chunks, warps 6..9 the odd ones
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    uint32_t epi_res_phase = 0;   // parity bits of this warp's two residual barriers
+    // ------------------------------------------------ consumer warpgroups: wgmma main loop (accumulator in registers), then the epilogue
+    setmaxnreg_inc<232>();
+    const int ew = warp - 4;                  // epilogue warp 0..7
+    const int wg = ew >> 2;                   // accumulator rows [64*wg, +64) of the tile
+    const int q = ew & 3;                     // warp of the warpgroup
+    const int lane_grp = 2 * wg + (q & 1);    // epilogue rows [32*lane_grp, +32): lane = row
+    const int chunk0 = (q >> 1) * 32;         // warps 0, 1 of a warpgroup take the even 32-column chunks, warps 2, 3 the odd ones
+    const uint32_t acc_wg = acc_base + (uint32_t)(wg * ACC_WG_BYTES);
+    const int tq = (threadIdx.x & 127);       // thread of the warpgroup
+    const int frag_row = 16 * q + (lane >> 2);
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    uint32_t epi_res_phase = 0;   // parity bits of this warp's residual barriers
     int vec_nblk = -1;            // column block whose bias / column-sum vectors sit in shared memory
     SegState ss = seg_init<SK>(p, tile0, tile_step, num_tiles);
     int t, kb0, kb1;
     bool first_seg = true;
+    // release a stage: this warpgroup is done reading it (in a pair, the peer's producer writes its B half into it too)
+    auto release = [&](int s) {
+      if (tq == 0) {
+        if (CL == 1) mbar_arrive(empty_bar(s));
+        else
+          for (int c = 0; c < CL; ++c) mbar_arrive_cluster(mapa_cluster(empty_bar(s), (uint32_t)c));
+      }
+    };
     while (seg_next<SK>(p, ss, tile_step, num_tiles, t, kb0, kb1)) {
       const int b = t / tiles_per_batch;
       const int r = t - b * tiles_per_batch;
@@ -358,7 +300,68 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const bool row_ok = row < p.M;
       const int n0 = n_blk * BN;
 
-      const uint32_t taddr = tmem_base + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)(acc * BN);
+      // ---- main loop: the MMAs of k-block kb are in flight while the stage of kb-1 is released
+      {
+        int prev = -1;
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(full_bar(stage), phase);
+          if (first_seg && kb == kb0 && ew == 0 && lane == 0) GEMM_STAMP(3);
+          const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES + (uint32_t)(wg * 64 * BK * 2);
+          const uint64_t adesc = wgmma_desc_k_sw128(sa);
+          const uint64_t bdesc = wgmma_desc_k_sw128(smem_base + stage * Cfg::STAGE_BYTES + A_STAGE_BYTES);
+          wgmma_fence_regs<BN / 2>(acc);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k)   // advance 16 fp16 = 32 B inside the 128B swizzle atom: +2 in the (addr >> 4) field
+            wgmma_ss_n<BN>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), ((kb - kb0) | k) != 0);
+          wgmma_commit();
+          wgmma_wait<1>();
+          wgmma_fence_regs<BN / 2>(acc);
+          if (prev >= 0) release(prev);
+          prev = stage;
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1u;
+          }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_regs<BN / 2>(acc);
+        if (prev >= 0) release(prev);
+      }
+      if (ew == 0 && lane == 0) {
+        if (first_seg) GEMM_STAMP(4);
+        GEMM_STAMP(5);                                 // overwritten every tile: the last tile's value survives
+      }
+      // columns [cp, cp + 64) of this warpgroup's accumulator -> shared memory (64 rows x ACC_LD), then every warp reads back its row x 32 columns
+      auto stage_acc = [&](int cp) {
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          if (8 * j >= cp && 8 * j < cp + 64) {
+            const uint32_t a = acc_wg + 4u * (uint32_t)(frag_row * ACC_LD + 8 * j - cp + 2 * (lane & 3));
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};\n" ::"r"(a), "f"(acc[4 * j]), "f"(acc[4 * j + 1]) : "memory");
+            asm volatile("st.shared.v2.f32 [%0], {%1, %2};\n" ::"r"(a + 8u * ACC_LD * 4u), "f"(acc[4 * j + 2]), "f"(acc[4 * j + 3]) : "memory");
+          }
+        }
+      };
+      auto load_acc = [&](uint32_t (&v)[32]) {
+        const uint32_t a = acc_wg + 4u * (uint32_t)(((q & 1) * 32 + lane) * ACC_LD + chunk0);
+#pragma unroll
+        for (int i = 0; i < 32; i += 4) {
+          const uint4 u = lds128(a + 4u * (uint32_t)i);
+          v[i] = u.x, v[i + 1] = u.y, v[i + 2] = u.z, v[i + 3] = u.w;
+        }
+      };
+      const int col_end = min(p.N, n0 + BN);   // columns of this tile that exist
+      // walk the 64-column slices of the accumulator (warpgroup-uniform); fn(c) handles this warp's 32-column chunk c when it exists
+      auto for_each_chunk = [&](auto&& fn) {
+        for (int cp = 0; cp < BN && n0 + cp < col_end; cp += 64) {
+          stage_acc(cp);
+          named_bar_sync(2 + wg, 128);
+          const int c = cp + chunk0;
+          if (c < BN && n0 + c < col_end) fn(c);
+          named_bar_sync(2 + wg, 128);           // the slice is consumed before the next one overwrites it
+        }
+      };
 
       const float bm = (p.bias_m != nullptr && row_ok) ? p.bias_m[row] : 0.f;
       float ln_rstd = 1.f, ln_nmr = 0.f;       // folded LayerNorm: x = rstd * acc + (-mean * rstd) * colsum[n]
@@ -367,8 +370,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         if (p.ln_parts > 0) {      // partial sums of the row, one per 32-column chunk of the producing GEMM, added in chunk order
           float s1 = 0.f, s2 = 0.f;
           for (int k = 0; k < p.ln_parts; ++k) {
-            const float2 q = __ldcg(p.ln_stats + (long long)k * p.M + row);
-            s1 += q.x, s2 += q.y;
+            const float2 qq = __ldcg(p.ln_stats + (long long)k * p.M + row);
+            s1 += qq.x, s2 += qq.y;
           }
           const float mean = s1 * p.ln_inv_cols;
           mr = make_float2(mean, rsqrtf(fmaxf(s2 * p.ln_inv_cols - mean * mean, 0.f) + p.ln_eps));
@@ -384,9 +387,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       const float* bg = (p.bias_g != nullptr && row_ok && !bg_vec) ? p.bias_g + (long long)(row / p.bias_g_rows) * p.N : nullptr;
       const int rrow = p.res_row_mod ? (row % p.res_row_mod) : row;
 
-      const int col_end = min(p.N, n0 + BN);   // columns of this tile that exist
       // ---- TMA epilogue state: tiles of 32 rows x RB bytes in this warp's staging area, XOR-swizzled like the tensor maps
-      const int ew = warp - 2;
       const uint32_t stg_out = epi_base + (uint32_t)(ew * p.epi_warp_bytes), stg_res = stg_out + (uint32_t)p.epi_out_bytes;
       const int RB = p.epi_row_bytes;
       const uint32_t tile_bytes = 32u * (uint32_t)RB;
@@ -411,30 +412,18 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       constexpr int BNP = (BN + 31) & ~31;                      // scratch row stride: the last 32-column chunk of a tile may reach past BN
       const size_t sk_tile_elems = (size_t)BM * BNP;
       if (sk_partial) {
-        mbar_wait_relaxed(tfull_bar(acc), acc_phase);
-        tc_fence_after();
         // layout of a slot: [BNP / 4 column quads][128 rows][4 floats]: the 32 lanes (= rows) of a store cover 512 contiguous bytes
         float* dst = p.sk_scratch + ((size_t)my_cluster * CL + crank) * sk_tile_elems + (size_t)(lane_grp * 32 + lane) * 4;
-#pragma unroll 1
-        for (int c = chunk0; c < BN; c += 64) {
-          if (n0 + c >= col_end) break;
-          __syncwarp();
+        for_each_chunk([&](int c) {
           uint32_t v[32];
-          tmem_ld32(taddr + (uint32_t)c, v);
-          tmem_ld_wait();
+          load_acc(v);
 #pragma unroll
           for (int i = 0; i < 32; i += 4) *(uint4*)(dst + (size_t)((c + i) >> 2) * (BM * 4)) = make_uint4(v[i], v[i + 1], v[i + 2], v[i + 3]);
-        }
+        });
         __threadfence();                                        // my stores are visible device-wide before the flag
-        tc_fence_before();
         __syncwarp();
-        if (lane == 0) {
+        if (lane == 0)
           asm volatile("st.release.gpu.global.u32 [%0], %1;\n" ::"l"(p.sk_flags + ((size_t)my_cluster * CL + crank) * EPI_WARPS + ew), "r"(1u) : "memory");
-          if (CL == 1) mbar_arrive(tempty_bar(acc));
-          else mbar_arrive_cluster(mapa_cluster(tempty_bar(acc), 0));
-        }
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1u;
         first_seg = false;
         continue;
       }
@@ -445,18 +434,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         while (sk_last + 1 < tile_step && (long long)(sk_last + 1) * total / tile_step < tile_end) ++sk_last;
       }
       if (tma_res && lane == 0)
-        for (int k = 0; k < nres && k < n_chunks; ++k) issue_res(k);  // in flight while the main loop of this tile is still running
-      // column vectors of this tile -> shared memory (while the main loop is still running): the chunk loop then reads them with broadcast
-      // 128-bit shared loads instead of 16 dependent L1/L2 round trips per chunk, which is what the short-K epilogues were waiting on
-#ifdef SEEDX_GEMM_NO_VEC
-      const bool use_vec = false;
-#else
+        for (int k = 0; k < nres && k < n_chunks; ++k) issue_res(k);
+      // column vectors of this tile -> shared memory: the chunk loop then reads them with broadcast 128-bit shared loads instead of dependent
+      // L1/L2 round trips per chunk
       const int vec_key = n_blk + (bg_vec ? (bg_grp + 1) * 65536 : 0);
       const bool use_vec = (p.bias_n != nullptr || p.ln_stats != nullptr || bg_vec) && vec_key != vec_nblk;   // consecutive tiles of a CTA mostly differ in m only
-#endif
       if (use_vec) {
         vec_nblk = vec_key;
-        asm volatile("bar.sync 1, %0;\n" ::"n"(EPI_WARPS * 32) : "memory");      // every epilogue warp has finished reading the previous tile's vectors
+        named_bar_sync(1, EPI_WARPS * 32);      // every epilogue warp has finished reading the previous tile's vectors
         for (int i = ew * 32 + lane; i < BN; i += EPI_WARPS * 32) {
           const bool in = n0 + i < col_end;
           float bv = (p.bias_n != nullptr && in) ? __ldg(p.bias_n + n0 + i) : 0.f;
@@ -465,15 +450,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           asm volatile("st.shared.f32 [%0], %1;\n" ::"r"(vec_base + 4u * (uint32_t)i), "f"(bv) : "memory");
           if (p.ln_stats != nullptr) asm volatile("st.shared.f32 [%0], %1;\n" ::"r"(vec_base + 1024u + 4u * (uint32_t)i), "f"(cv) : "memory");
         }
-        asm volatile("bar.sync 1, %0;\n" ::"n"(EPI_WARPS * 32) : "memory");
+        named_bar_sync(1, EPI_WARPS * 32);
       }
       int kchunk = 0;
-      mbar_wait_relaxed(tfull_bar(acc), acc_phase);   // accumulator of this tile complete
-      if (warp == 2 && lane == 0) {
-        if (first_seg) GEMM_STAMP(4);
-        GEMM_STAMP(5);                                 // overwritten every tile: the last tile's value survives
-      }
-      tc_fence_after();
       if (sk_owner) {                                  // the contributors wrote their partials at the START of their work: normally long done
         for (int cc = my_cluster + 1; cc <= sk_last; ++cc) {
           const unsigned* f = p.sk_flags + ((size_t)cc * CL + crank) * EPI_WARPS + ew;
@@ -485,45 +464,23 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
         __syncwarp();
       }
-#pragma unroll 1
-      for (int c = chunk0; c < BN; c += 64) {
-        if (n0 + c >= col_end) break;  // warp-uniform
-        __syncwarp();              // tcgen05.ld is warp-collective: reconverge after the predicated stores
+      for_each_chunk([&](int c) {
         uint32_t v[32];
-        tmem_ld32(taddr + (uint32_t)c, v);
-        tmem_ld_wait();
+        load_acc(v);
         if (sk_owner) {            // partial sums of the later k-blocks, added in cluster order (fixed order: reproducible)
           for (int cc = my_cluster + 1; cc <= sk_last; ++cc) {
             const float* src = p.sk_scratch + ((size_t)cc * CL + crank) * sk_tile_elems + (size_t)(lane_grp * 32 + lane) * 4;
 #pragma unroll
             for (int i = 0; i < 32; i += 4) {
-              const float4 q = __ldcg((const float4*)(src + (size_t)((c + i) >> 2) * (BM * 4)));
-              v[i] = __float_as_uint(__uint_as_float(v[i]) + q.x), v[i + 1] = __float_as_uint(__uint_as_float(v[i + 1]) + q.y);
-              v[i + 2] = __float_as_uint(__uint_as_float(v[i + 2]) + q.z), v[i + 3] = __float_as_uint(__uint_as_float(v[i + 3]) + q.w);
+              const float4 qv = __ldcg((const float4*)(src + (size_t)((c + i) >> 2) * (BM * 4)));
+              v[i] = __float_as_uint(__uint_as_float(v[i]) + qv.x), v[i + 1] = __float_as_uint(__uint_as_float(v[i + 1]) + qv.y);
+              v[i + 2] = __float_as_uint(__uint_as_float(v[i + 2]) + qv.z), v[i + 3] = __float_as_uint(__uint_as_float(v[i + 3]) + qv.w);
             }
           }
         }
         float x[32];
         const int col0 = n0 + c;
-#ifdef SEEDX_GEMM_NO_VEC
-        {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) x[i] = fmaf(__uint_as_float(v[i]), p.alpha, bm);
-          if (p.bias_n != nullptr) {
-#pragma unroll
-            for (int i = 0; i < 32; i += 4) {
-              if (col0 + i + 4 <= col_end) {
-                const float4 q = __ldg((const float4*)(p.bias_n + col0 + i));
-                x[i] += q.x, x[i + 1] += q.y, x[i + 2] += q.z, x[i + 3] += q.w;
-              }
-            }
-          }
-        }
-        constexpr bool kVec = false;
-#else
-        constexpr bool kVec = true;
-#endif
-        if (kVec && p.ln_stats != nullptr) {
+        if (p.ln_stats != nullptr) {
           // folded LayerNorm (alpha = 1, no bias_m: host check): x = rstd * acc + (bias - rstd * mean * colsum) -> two FFMAs per value
 #pragma unroll
           for (int i = 0; i < 32; i += 4) {
@@ -533,14 +490,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             x[i + 2] = fmaf(__uint_as_float(v[i + 2]), ln_rstd, fmaf(ln_nmr, __uint_as_float(qc.z), __uint_as_float(qb.z)));
             x[i + 3] = fmaf(__uint_as_float(v[i + 3]), ln_rstd, fmaf(ln_nmr, __uint_as_float(qc.w), __uint_as_float(qb.w)));
           }
-        } else if (kVec && (p.bias_n != nullptr || bg_vec)) {
+        } else if (p.bias_n != nullptr || bg_vec) {
 #pragma unroll
           for (int i = 0; i < 32; i += 4) {
             const uint4 qb = lds128(vec_base + 4u * (uint32_t)(c + i));
             x[i] = fmaf(__uint_as_float(v[i]), p.alpha, __uint_as_float(qb.x) + bm), x[i + 1] = fmaf(__uint_as_float(v[i + 1]), p.alpha, __uint_as_float(qb.y) + bm);
             x[i + 2] = fmaf(__uint_as_float(v[i + 2]), p.alpha, __uint_as_float(qb.z) + bm), x[i + 3] = fmaf(__uint_as_float(v[i + 3]), p.alpha, __uint_as_float(qb.w) + bm);
           }
-        } else if (kVec) {
+        } else {
 #pragma unroll
           for (int i = 0; i < 32; ++i) x[i] = fmaf(__uint_as_float(v[i]), p.alpha, bm);
         }
@@ -587,17 +544,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
               for (int j = 0; j < 8; ++j) {
                 if (4 * j < nvals) {
-                  const uint4 q = lds128(rrow_addr + (((uint32_t)j ^ sw) << 4));
-                  x[4 * j] += __uint_as_float(q.x), x[4 * j + 1] += __uint_as_float(q.y);
-                  x[4 * j + 2] += __uint_as_float(q.z), x[4 * j + 3] += __uint_as_float(q.w);
+                  const uint4 qv = lds128(rrow_addr + (((uint32_t)j ^ sw) << 4));
+                  x[4 * j] += __uint_as_float(qv.x), x[4 * j + 1] += __uint_as_float(qv.y);
+                  x[4 * j + 2] += __uint_as_float(qv.z), x[4 * j + 3] += __uint_as_float(qv.w);
                 }
               }
             } else {
 #pragma unroll
               for (int j = 0; j < 4; ++j) {
                 if (8 * j < nvals) {
-                  const uint4 q = lds128(rrow_addr + (((uint32_t)j ^ sw) << 4));
-                  const __half2* h = (const __half2*)&q;
+                  const uint4 qv = lds128(rrow_addr + (((uint32_t)j ^ sw) << 4));
+                  const __half2* h = (const __half2*)&qv;
 #pragma unroll
                   for (int e = 0; e < 4; ++e) {
                     const float2 f = __half22float2(h[e]);
@@ -627,11 +584,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
               if (8 * j < nvals) {
-                uint4 q;
-                __half2* h = (__half2*)&q;
+                uint4 qv;
+                __half2* h = (__half2*)&qv;
 #pragma unroll
                 for (int e = 0; e < 4; ++e) h[e] = __floats2half2_rn(x[8 * j + 2 * e], x[8 * j + 2 * e + 1]);
-                sts128(orow_addr + (((uint32_t)j ^ sw) << 4), q);
+                sts128(orow_addr + (((uint32_t)j ^ sw) << 4), qv);
               }
             }
           }
@@ -652,19 +609,19 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             const uint32_t tb = stg_out + (uint32_t)ob * tile_bytes + (uint32_t)((lane & 7) * 2);
             float s1 = 0.f, s2 = 0.f;
 #pragma unroll
-            for (int r = 0; r < 32; ++r) {
-              const uint32_t a = tb + (uint32_t)(r * 64) + ((((uint32_t)lane >> 3) ^ (((uint32_t)r >> 1) & 3u)) << 4);
+            for (int rr = 0; rr < 32; ++rr) {
+              const uint32_t a = tb + (uint32_t)(rr * 64) + ((((uint32_t)lane >> 3) ^ (((uint32_t)rr >> 1) & 3u)) << 4);
               unsigned short hv;
               asm volatile("ld.shared.u16 %0, [%1];\n" : "=h"(hv) : "r"(a));
-              const float v = __half2float(__ushort_as_half(hv));
-              s1 += v, s2 = fmaf(v, v, s2);
+              const float fv = __half2float(__ushort_as_half(hv));
+              s1 += fv, s2 = fmaf(fv, fv, s2);
             }
             if (col0 + lane < col_end) p.col_part[(long long)(row_base >> 5) * p.N + col0 + lane] = make_float2(s1, s2);
           }
-          continue;
+          return;
         }
         const int n_out = p.gated ? (col_end >> 1) : col_end;  // output columns of this tile end here
-        if (!row_ok) continue;
+        if (!row_ok) return;
         const bool full = (ocol0 + nvals <= n_out) && p.vec_ok;
         if (p.residual != nullptr) {
           if (p.res_f32) {
@@ -673,8 +630,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
               for (int i = 0; i < 32; i += 4) {
                 if (i < nvals) {
-                  const float4 q = *(const float4*)(rp + i);
-                  x[i] += q.x, x[i + 1] += q.y, x[i + 2] += q.z, x[i + 3] += q.w;
+                  const float4 qv = *(const float4*)(rp + i);
+                  x[i] += qv.x, x[i + 1] += qv.y, x[i + 2] += qv.z, x[i + 3] += qv.w;
                 }
               }
             } else {
@@ -688,8 +645,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
               for (int i = 0; i < 32; i += 8) {
                 if (i < nvals) {
-                  const uint4 q = *(const uint4*)(rp + i);
-                  const __half2* h = (const __half2*)&q;
+                  const uint4 qv = *(const uint4*)(rp + i);
+                  const __half2* h = (const __half2*)&qv;
 #pragma unroll
                   for (int j = 0; j < 4; ++j) {
                     const float2 f = __half22float2(h[j]);
@@ -721,11 +678,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
             for (int i = 0; i < 32; i += 8) {
               if (i < nvals) {
-                uint4 q;
-                __half2* h = (__half2*)&q;
+                uint4 qv;
+                __half2* h = (__half2*)&qv;
 #pragma unroll
                 for (int j = 0; j < 4; ++j) h[j] = __floats2half2_rn(x[i + 2 * j], x[i + 2 * j + 1]);
-                *(uint4*)(dp + i) = q;
+                *(uint4*)(dp + i) = qv;
               }
             }
           } else {
@@ -734,12 +691,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               if (i < nvals && ocol0 + i < n_out) dp[i] = __float2half_rn(x[i]);
           }
         }
-      }
-      tc_fence_before();
+      });
       __syncwarp();
       if (p.row_stats_out != nullptr && row_base < p.M) {
-        // my partials of this slab are written: take a ticket.  A slab receives 2 * n_blocks deliveries (the even- and the odd-chunk warp of its lane
-        // quarter, once per column block); the last one reduces the slab.
+        // my partials of this slab are written: take a ticket.  A slab receives 2 * n_blocks deliveries (the even- and the odd-chunk warp of its
+        // rows, once per column block); the last one reduces the slab.
         __threadfence();
         __syncwarp();
         unsigned last = 0;
@@ -752,8 +708,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             float s1 = 0.f, s2 = 0.f;
 #pragma unroll 4
             for (int k = 0; k < parts; ++k) {
-              const float2 q = __ldcg(p.row_part + (long long)k * p.M + row);
-              s1 += q.x, s2 += q.y;
+              const float2 qq = __ldcg(p.row_part + (long long)k * p.M + row);
+              s1 += qq.x, s2 += qq.y;
             }
             const float inv = 1.0f / (float)p.N;
             const float mean = s1 * inv;
@@ -762,29 +718,17 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           if (lane == 0) p.row_tickets[row_base >> 5] = 0u;
         }
       }
-      if (lane == 0) {
-        if (CL == 1) mbar_arrive(tempty_bar(acc));
-        else mbar_arrive_cluster(mapa_cluster(tempty_bar(acc), 0));  // the leader's MMA thread owns the accumulator hand-shake
-        if (sk_owner)                                                // flags back to 0: one writer and one reader each, nobody else looks at them
-          for (int cc = my_cluster + 1; cc <= sk_last; ++cc) p.sk_flags[((size_t)cc * CL + crank) * EPI_WARPS + ew] = 0u;
-      }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1u;
+      if (lane == 0 && sk_owner)                       // flags back to 0: one writer and one reader each, nobody else looks at them
+        for (int cc = my_cluster + 1; cc <= sk_last; ++cc) p.sk_flags[((size_t)cc * CL + crank) * EPI_WARPS + ew] = 0u;
       first_seg = false;
     }
     if (p.tma_epi && lane == 0) bulk_wait_read<0>();  // shared memory stays alive until the last TMA store has read it
-    if (warp == 2 && lane == 0) GEMM_STAMP(6);
+    if (ew == 0 && lane == 0) GEMM_STAMP(6);
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (CL > 1) cluster_sync_all();  // no CTA leaves while its peer may still read its shared memory / arrive on its barriers
-  if (warp == 1) {
-    tc_fence_after();
-    if (CL == 1) tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-    else tmem_dealloc_2sm<Cfg::TMEM_COLS>(tmem_base);
-    if (lane == 0) GEMM_STAMP(7);
-  }
+  if (CL > 1) cluster_sync_all();  // no CTA leaves while its peer may still write into its shared memory / arrive on its barriers
+  if (threadIdx.x == 0) GEMM_STAMP(7);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -794,9 +738,8 @@ void count_launch();
 
 // stream-K fix-up workspace (seedx_gemm_set_workspace): flags first (zeroed by the caller), partial tiles behind them
 static int g_gemm_stream_k = 1;       // 0 = off, 1 = auto, 2 = whenever legal (tests)
-static int g_sk_min_kblocks = 90;     // auto mode: shortest K (in 64-element blocks) that is split: the 3x3 convs from 640 channels (K >= 5760).  The K = 5120
-                                      // feed-forward output GEMM (80 blocks) runs in the same time either way (A/B: 63.3 vs 63.0-63.9 ms per forward) but its
-                                      // stream-K order defeats the L2 reuse of A: 400 MB instead of 75 MB of DRAM reads per launch (ncu launch lists)
+static int g_sk_min_kblocks = 90;     // auto mode: shortest K (in 64-element blocks) that is split: the 3x3 convs from 640 channels (K >= 5760).  Shorter K
+                                      // gains little from balancing, and the stream-K order defeats the L2 reuse of A
 static float* g_sk_scratch = nullptr;
 static size_t g_sk_scratch_bytes = 0;
 static unsigned* g_sk_flags = nullptr;
@@ -806,7 +749,7 @@ template <int BN, int CL>
 static int launch_gemm_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& td, const CUtensorMap& tr, const GemmParams& p_in,
                           cudaStream_t st) {
   using Cfg = TileCfg<BN, CL>;
-  // stream-K kernels exist for CTA pairs with 32-column-multiple tiles of at least 128 columns (where the schedule is ever chosen)
+  // stream-K kernels exist for cluster pairs with 32-column-multiple tiles of at least 128 columns (where the schedule is ever chosen)
   constexpr bool kHasSK = (CL == 2) && (BN % 32 == 0) && (BN >= 128);
   static bool attr_done = false;
   if (!attr_done) {
@@ -815,16 +758,39 @@ static int launch_gemm_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CU
     attr_done = true;
   }
   GemmParams p = p_in;
-  const int epi_bytes = EPI_WARPS * p.epi_warp_bytes;
+  int epi_bytes = EPI_WARPS * p.epi_warp_bytes;
   const int tail_bytes = 512 + (p.bias_n != nullptr || p.ln_stats != nullptr || p.bias_g != nullptr ? VEC_BYTES : 0) + (p.ln_stats != nullptr ? VEC_BYTES : 0);
   p.stages = Cfg::stages_for(epi_bytes, tail_bytes);
+  if (p.stages < 3 && p.tma_epi && p.epi_warp_bytes > 32 * p.epi_row_bytes * (p.epi_res_bytes ? 2 : 1)) {
+    // the short-K staging (several boxes in flight per warp) would leave a wide tile fewer than three pipeline stages: one box each
+    p.epi_out_bytes = 32 * p.epi_row_bytes;
+    p.epi_res_bytes = p.epi_res_bytes ? 32 * p.epi_row_bytes : 0;
+    p.epi_warp_bytes = p.epi_out_bytes + p.epi_res_bytes;
+    epi_bytes = EPI_WARPS * p.epi_warp_bytes;
+    p.stages = Cfg::stages_for(epi_bytes, tail_bytes);
+  }
   if (p.stages < 2) {
     set_error("seedx_gemm_f16: tile %dx%d does not fit in shared memory with %d B of epilogue staging", BM * CL, BN, epi_bytes);
     return 5;
   }
   const int smem_bytes = Cfg::smem_for(p.stages, epi_bytes, tail_bytes);
   const int groups = ((p.m_blocks + CL - 1) / CL) * p.n_blocks * p.batch;
-  const int max_clusters = num_sms() / CL;
+  int max_clusters = num_sms() / CL;
+  if (CL > 1) {
+    // a cluster must fit in one GPC: fewer pairs than num_sms / 2 may be co-resident, and a persistent grid larger than that runs a second wave
+    static int occ_smem = -1, occ_clusters = 0;
+    if (occ_smem != smem_bytes) {
+      cudaLaunchConfig_t q{};
+      q.gridDim = dim3(max_clusters * CL), q.blockDim = dim3(GEMM_THREADS), q.dynamicSmemBytes = smem_bytes;
+      cudaLaunchAttribute qa[1];
+      qa[0].id = cudaLaunchAttributeClusterDimension;
+      qa[0].val.clusterDim.x = CL, qa[0].val.clusterDim.y = 1, qa[0].val.clusterDim.z = 1;
+      q.attrs = qa, q.numAttrs = 1;
+      SEEDX_CUDA(cudaOccupancyMaxActiveClusters(&occ_clusters, gemm_tc_kernel<BN, CL, false>, &q));
+      occ_smem = smem_bytes;
+    }
+    if (occ_clusters > 0 && occ_clusters < max_clusters) max_clusters = occ_clusters;
+  }
   const int grid = (groups < max_clusters ? groups : max_clusters) * CL;
   // Stream-K when the last wave of whole tiles would leave SMs idle: every cluster gets total/clusters k-iterations instead of whole tiles.
   // Needs the fix-up workspace, at least 4 iterations per cluster (no empty cluster, a partial is worth its round trip) and a tile that
@@ -836,8 +802,7 @@ static int launch_gemm_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CU
     const int rem = groups % clusters;
     const bool idle_tail = rem != 0 && (double)(clusters - rem) / clusters / ((groups + clusters - 1) / clusters) > 0.04;   // > 4 % of the launch idle
     const size_t need = (size_t)clusters * CL * BM * ((BN + 31) & ~31) * sizeof(float);
-    // measured on B200 (profiles/r02_unet_forward_launches_*): the fix-up round trip pays off from ~100 k-blocks per tile (the 3x3 convs with
-    // C >= 1280, K = 11 520: -10 ... -17 %), not for the K = 1280 ... 5120 transformer GEMMs, whose whole launch is 30 - 100 us
+    // the fix-up round trip of a partial tile (2 x 128 x BN fp32 through L2) is only worth it for long K (g_sk_min_kblocks)
     const bool long_k = p.k_blocks >= g_sk_min_kblocks;
     if (kHasSK && g_gemm_stream_k != 0 && g_sk_scratch != nullptr && need <= g_sk_scratch_bytes && total >= 4LL * clusters && groups > clusters &&
         ((idle_tail && long_k) || g_gemm_stream_k == 2)) {
@@ -871,7 +836,7 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
 }
 
 static unsigned long long* g_gemm_dbg = nullptr;
-static int g_gemm_cluster = 1;  // 0 = never cluster, 1 = auto, 2 = always when legal
+static int g_gemm_cluster = 1;  // 0 = never cluster, 1 = auto (single-CTA tiles), 2 = always when legal
 static int g_gemm_tma_epi = 1;  // 0 = row-per-thread direct stores, 1 = TMA-store epilogue when eligible
 
 static const int kTileN[] = {64, 96, 128, 144, 160, 192, 208, 224, 240, 256};
@@ -883,25 +848,34 @@ static bool valid_tile_n(int bn) {
 }
 
 // Pick the N tile that minimises a simple cycle model of the persistent kernel:
-//   waves = ceil(tiles / SMs); per tile max(MMA issue, epilogue drain) cycles; plus the un-overlapped epilogue of the last tile.
-// MMA: 128 x BN x 16 per instruction = BN/2 cycles, but never faster than shared memory can feed A+B; the effective operand
-// bandwidth measured on B200 (8192^3: BN=128 runs at 0.71x the BN=256 rate) is ~91 B/clk.
+//   waves = ceil(tiles / SMs); per tile MMA cycles + epilogue cycles (the consumer warpgroups run both in turn).
+// MMA: a 128 x BN x 16 step is BN cycles at the dense fp16 rate of an H100 SM (2048 FMA/clk), divided by the rate a tile width reaches
+// relative to the 256-wide tile.  Measured on an H100 SXM at 700 W, 8192^3 single-CTA launches (256 wide: 616 TFLOP/s): narrower tiles
+// re-read A more often per FLOP and leave more stages' worth of latency exposed, widths that are not one wgmma instruction issue several.
+struct TileRate {
+  int bn;
+  double rate;
+};
+static const TileRate kAutoTiles[] = {{128, 0.82}, {160, 0.78}, {192, 0.94}, {224, 0.73}, {256, 1.0}};
+
 static int choose_tile_n(int m_tiles, int N, int k_blocks, bool heavy_epilogue, bool only32) {
   const int sms = num_sms();
   double best = 1e30;
   int best_bn = 256;
-  for (int bn : kTileN) {
+  for (const TileRate& tr : kAutoTiles) {
+    const int bn = tr.bn;
     if (only32 && bn % 32 != 0) continue;  // the TMA epilogue stores whole 32-column chunks
     const int n_blocks = (N + bn - 1) / bn;
     const long long tiles = (long long)m_tiles * n_blocks;
-    // stream-K (workspace present): a launch of more than one wave costs its fractional number of waves plus the partial-tile round trip
-    const bool sk = (bn % 32 == 0 && bn >= 128) && g_gemm_stream_k != 0 && g_sk_scratch != nullptr && tiles > sms && (long long)tiles * k_blocks >= 4LL * sms &&
+    // stream-K (cluster pairs forced, workspace present): a launch of more than one wave costs its fractional number of waves plus the partial-tile round trip
+    const bool sk = (bn % 32 == 0 && bn >= 128) && g_gemm_cluster == 2 && g_gemm_stream_k != 0 && g_sk_scratch != nullptr && tiles > sms &&
+                    (long long)tiles * k_blocks >= 4LL * sms &&
                     (k_blocks >= g_sk_min_kblocks || g_gemm_stream_k == 2);
     const double waves = sk ? (double)tiles / sms + 0.12 : (double)((tiles + sms - 1) / sms);
-    const double mma_k16 = fmax(bn / 2.0, (4096.0 + 32.0 * bn) / 91.0);
+    const double mma_k16 = bn / tr.rate;
     const double mma = k_blocks * 4.0 * mma_k16;
     const double epi = bn * (heavy_epilogue ? 14.0 : 8.0) + 300.0;
-    const double cost = waves * (fmax(mma, epi) + 150.0) + epi;
+    const double cost = waves * (mma + epi + 150.0);
     if (cost < best - 1e-9 || (fabs(cost - best) <= 1e-9 && bn > best_bn)) best = cost, best_bn = bn;
   }
   return best_bn;
@@ -1017,10 +991,9 @@ extern "C" int seedx_gemm_f16(const seedx_gemm_args* a, void* stream) {
     uint64_t bstride = bb ? (uint64_t)a->strideB * 2 : (uint64_t)a->ldb * 2 * (uint64_t)a->N;
     SEEDX_REQUIRE(bstride % 16 == 0, "seedx_gemm_f16: strideB must be a multiple of 8 elements");
     uint64_t strides[2] = {(uint64_t)a->ldb * 2, bstride};
-    // CTA pairs (cta_group::2) when every SM still gets work and the B tile splits into two 16-row-aligned halves
-    const long long groups2 = (long long)((p.m_blocks + 1) / 2) * ((a->N + bn - 1) / bn) * a->batch;
-    cl = (g_gemm_cluster != 0 && p.m_blocks >= 2 && bn % 32 == 0 && groups2 >= num_sms() / 2) ? 2 : 1;
-    if (g_gemm_cluster == 2 && p.m_blocks >= 2 && bn % 32 == 0) cl = 2;  // forced (tests)
+    // cluster pairs (B tile multicast in two halves, 16-row aligned) only when forced: on an H100 SXM (700 W) they measured about half the
+    // single-CTA rate on every shape tried (8192 x {10240, 1280, 8192} x {1280, 5120, 8192}), so auto mode keeps single-CTA tiles
+    if (g_gemm_cluster == 2 && p.m_blocks >= 2 && bn % 32 == 0) cl = 2;
     // a single CTA with residual staging (96 KB) keeps only 2 stages of a 256-wide tile: use a narrower tile there
     if (cl == 1 && tma_epi && a->residual && bn > 160 && a->tile_n == 0) bn = 160;
     uint32_t box[3] = {BK, (uint32_t)(bn / cl), 1};

@@ -47,7 +47,7 @@ int num_sms() {
     if (cudaGetDevice(&dev) == cudaSuccess && cudaGetDeviceProperties(&prop, dev) == cudaSuccess)
       n = prop.multiProcessorCount;
     else
-      n = 148;
+      n = 132;
   }
   return n;
 }

@@ -107,7 +107,7 @@ def get_peft_model_with_resize_embedding(model, peft_config=None, model_id=None,
     ``model``: a built LlamaForCausalLM or its `_target_` mapping.  Exactly one of ``peft_config`` (adapters arrive later with the agent
     checkpoint, README.md:150-160) and ``model_id`` (a PEFT adapter directory: adapter_config.json + adapter_model.bin/.safetensors, merged
     now) must be given.  ``vocab_size``: rows are appended to both embeddings — input rows = mean of the old rows, output rows = 3x the
-    mean (peft_models.py:62-82).  ``torch_dtype`` is accepted for signature parity; operands are fp16 (DESIGN.md §4)."""
+    mean (peft_models.py:62-82).  ``torch_dtype`` is accepted for signature parity; operands are fp16."""
     if isinstance(model, dict) and "_target_" in model:
         from .compat import instantiate
         model = instantiate(model)

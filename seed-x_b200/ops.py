@@ -38,7 +38,7 @@ _workspace = {}
 
 def _ensure_workspace(device):
     """stream-K fix-up workspace of seedx_gemm_f16 (include/seedx.h: seedx_gemm_set_workspace), one per process: 16 KB of flags (zero) + room for
-    one fp32 partial tile per cluster (148 x 128 x 256 x 4 B = 19.4 MB).  Allocated on the first GEMM — before any CUDA-graph capture, which
+    one fp32 partial tile per CTA (132 x 128 x 256 x 4 B = 17.3 MB).  Allocated on the first GEMM — before any CUDA-graph capture, which
     always follows an eager warm-up pass."""
     key = torch.device(device).index if torch.device(device).index is not None else torch.cuda.current_device()
     if key not in _workspace:

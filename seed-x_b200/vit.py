@@ -6,7 +6,7 @@ same constructor keywords, ``from_pretrained``, ``eval()``, ``to()``, ``__call__
 and it ingests the reference state-dict key names (SURVEY.md A.5).
 
 Device data layout (HBM): activations are token-major [N*S, C]; the residual stream is fp32, GEMM operands fp16,
-accumulation fp32 (DESIGN.md §3).  Input-independent pieces (bicubic-resized position tables, the pooled query
+accumulation fp32.  Input-independent pieces (bicubic-resized position tables, the pooled query
 projection) are computed once at load / first use.
 """
 import math
@@ -82,7 +82,7 @@ class ResamplerWeights:
 
 
 class VisionTransformerWithAttnPool:
-    """B200-native drop-in for the reference visual encoder (forward only)."""
+    """Drop-in for the reference visual encoder (forward only)."""
 
     def __init__(self, image_size, patch_size, width, layers, heads, mlp_ratio, n_queries=256, output_dim=512,
                  patch_pos=False, **kwargs):
@@ -112,7 +112,7 @@ class VisionTransformerWithAttnPool:
 
     def to(self, device=None, dtype=None, **kw):
         if dtype is not None and dtype not in (torch.float16, torch.float32):
-            raise SeedxError("the B200 engine computes with fp16 operands / fp32 accumulate only")
+            raise SeedxError("the engine computes with fp16 operands / fp32 accumulate only")
         if dtype is not None:
             self.out_dtype = dtype
         return self

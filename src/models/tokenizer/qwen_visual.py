@@ -1,3 +1,3 @@
-"""`src.models.tokenizer.qwen_visual.*` -> B200 engine classes (reference: /root/reference/src/models/tokenizer/qwen_visual.py)."""
+"""`src.models.tokenizer.qwen_visual.*` -> H100 engine classes (reference: src/models/tokenizer/qwen_visual.py)."""
 from seedx_b200.agent import Resampler  # noqa: F401
 from seedx_b200.vit import VisionTransformerWithAttnPool  # noqa: F401

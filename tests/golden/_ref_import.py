@@ -1,13 +1,14 @@
-"""Import the UNMODIFIED reference modules from /root/reference on CPU (only in the build container; the GPU box has no
-/root/reference).  Three import stubs are needed (SURVEY.md §8c): deepspeed, transformers.deepspeed, xformers.ops."""
+"""Import the UNMODIFIED reference modules on CPU from the reference tree (SEEDX_REFERENCE, default /root/reference), where it exists.
+Three import stubs are needed (SURVEY.md §8c): deepspeed, transformers.deepspeed, xformers.ops."""
 import importlib
+import os
 import sys
 import types
 
 import torch
 import torch.nn.functional as F
 
-REF = "/root/reference"
+REF = os.environ.get("SEEDX_REFERENCE", "/root/reference")
 
 
 def install_stubs():

@@ -197,8 +197,8 @@ def test_vae_full_size_decode_and_encode_match_oracle(cpu_threads, force_upcast)
 # LLaMA at 13B width
 # ------------------------------------------------------------------------------------------------------------------------------------------
 def test_llama_13b_width_four_layers_prefill_and_greedy_match_oracle(cpu_threads):
-    """modeling_llama_xformer.py:643-746 at hidden 5120 / 40 heads / FFN 13824 / vocab 32330, 4 layers: prefill of P=174 rows (tcgen05 GEMMs +
-    causal tcgen05 attention at d=128) and 8 greedy tokens (GEMV token loop over the paged KV cache, CUDA graph)."""
+    """modeling_llama_xformer.py:643-746 at hidden 5120 / 40 heads / FFN 13824 / vocab 32330, 4 layers: prefill of P=174 rows (wgmma GEMMs +
+    causal wgmma attention at d=128) and 8 greedy tokens (GEMV token loop over the paged KV cache, CUDA graph)."""
     from oracle import llm as ollm
     from seedx_b200.llm import LLAMA_13B, LlamaForCausalLM
     cfg = dict(LLAMA_13B, layers=4)

@@ -1,4 +1,4 @@
-"""Parity of the tcgen05 GEMM / implicit-GEMM conv (seedx_gemm_f16) against a torch fp32 reference of the same op.
+"""Parity of the wgmma GEMM / implicit-GEMM conv (seedx_gemm_f16) against a torch fp32 reference of the same op.
 
 Tolerance: operands are fp16 (exactly representable in fp32), accumulation fp32 -> the only differences are the
 summation order and the final rounding to the output dtype: rel-Frobenius <= 2e-3 for fp16 out, 1e-5 for fp32 out.

@@ -26,19 +26,28 @@ def mk(shape, seed, scale=1.0):
     (2, 10, 4096, 4096, 64, False),    # UNet self-attention 64x64
     (8, 20, 1024, 1024, 64, False),    # UNet self-attention 32x32 at batch: enough items for the two-tile kernel
     (5, 16, 1024, 1024, 104, False),   # ViT MHSA, 5 views: two-tile kernel, padded head dim
-    (2, 20, 1024, 64, 64, False),      # UNet cross-attention: the 64 context tokens are one 64-key tcgen05 tile
+    (2, 20, 1024, 64, 64, False),      # UNet cross-attention: the 64 context tokens are one 64-key wgmma tile
     (8, 10, 4096, 64, 64, False),      # ... at the 64x64 level, bench batch
     (3, 5, 640, 48, 64, False),        # 64-key tile with 16 masked keys, ragged query tiles
     (2, 4, 256, 64, 40, False),        # head dim padded to 64 by TMA zero fill
     (2, 16, 64, 128, 64, False),       # perceiver
     (2, 16, 1, 65, 64, False),         # AttentionPool2d (single query)
     (1, 3, 77, 33, 72, False),
+    (2, 8, 64, 16, 64, False),         # the smallest problem of the wgmma kernel: one 64-row half tile, 16 keys of a 64-key tile
+    (1, 4, 300, 300, 104, True),       # causal, head dim 104 (two 64-column TMA chunks), ragged query and key tiles
+    (2, 3, 1000, 1000, 128, True),     # causal over eight 128-key tiles, ragged last query tile
+    (1, 2, 1000, 129, 64, False),      # 128-key tiles with one valid key in the last
+    (3, 2, 200, 65, 128, False),       # 65 keys: first size past the 64-key tile
+    (1, 1, 64, 4096, 8, False),        # head dim 8 zero-filled to 64
+    (2, 6, 4096, 64, 120, False),      # head dim 120, 64-key tile
+    (1, 5, 640, 640, 64, True),        # causal at the UNet head dim
+    (4, 4, 512, 300, 96, False),       # head dim 96
 ])
-@pytest.mark.parametrize("impl", ["tcgen05", "tcgen05_one_tile", "mma_sync"])
+@pytest.mark.parametrize("impl", ["wgmma", "mma_sync"])
 def test_attention(B, H, Sq, Sk, D, causal, impl):
     from seedx_b200 import ops
     from seedx_b200._lib import lib
-    lib().seedx_attention_set_impl({"tcgen05": 0, "tcgen05_one_tile": 2, "mma_sync": 1}[impl])
+    lib().seedx_attention_set_impl({"wgmma": 0, "mma_sync": 1}[impl])
     shared_q = (Sq == 256 and Sk == 1024)
     q = mk((1 if shared_q else B, Sq, H, D), 1).half()
     k = mk((B, Sk, H, D), 2).half()
@@ -51,19 +60,16 @@ def test_attention(B, H, Sq, Sk, D, causal, impl):
     lib().seedx_attention_set_impl(0)
     ref = F.scaled_dot_product_attention(qf, k.float().permute(0, 2, 1, 3), v.float().permute(0, 2, 1, 3), is_causal=causal, scale=scale)
     assert rel(o.permute(0, 2, 1, 3), ref) < 2e-3
-    if impl != "mma_sync" and Sq >= 128 and Sk <= 64 and Sk >= 16 and D <= 64 and not causal:
-        assert used == 2, "the 64-key tcgen05 tile should have handled this cross-attention shape, got %d" % used
-    if impl != "mma_sync" and Sq >= 128 and Sk >= 96 and D <= 128:
-        assert used in (2, 3), "a tcgen05 kernel should have handled this shape, got %d" % used
-        if impl == "tcgen05_one_tile":
-            assert used == 2
+    if impl == "wgmma" and Sq >= 64 and Sk >= 16 and D <= 128:
+        assert used == 2, "the wgmma kernel should have handled this shape, got %d" % used
+    if impl == "mma_sync":
+        assert used == 1
 
 
 @pytest.mark.parametrize("growth", [0.0, 1.5, 6.0])
 def test_attention_one_pass_softmax_redo(growth):
-    """The two-tile kernel exponentiates tiles after the first against the RUNNING maximum (one pass) and redoes a tile from the intact scores when a row
-    outgrew that reference by more than 2^8.  Keys whose magnitude rises with their index push later tiles above the running maximum: a little
-    (lazy rescale only), and by far more than 2^8 (redo path; fp16 P would be inf without it)."""
+    """Keys whose magnitude rises with their index push later key tiles above the running maximum of the online softmax: a little, and by far
+    more than 2^8 (fp16 P would be inf if a tile were exponentiated against a stale maximum)."""
     from seedx_b200 import ops
     from seedx_b200._lib import lib
     B, H, S, D = 8, 20, 1024, 64
@@ -73,7 +79,7 @@ def test_attention_one_pass_softmax_redo(growth):
     v = mk((B, S, H, D), 13).half()
     o = torch.empty((B, S, H, D), device="cuda", dtype=torch.float16)
     ops.attention(q.permute(0, 2, 1, 3), k.permute(0, 2, 1, 3), v.permute(0, 2, 1, 3), o.permute(0, 2, 1, 3), scale=D ** -0.5)
-    assert lib().seedx_attention_last_impl() == 3
+    assert lib().seedx_attention_last_impl() == 2
     ref = F.scaled_dot_product_attention(q.float().permute(0, 2, 1, 3), k.float().permute(0, 2, 1, 3), v.float().permute(0, 2, 1, 3), scale=D ** -0.5)
     assert torch.isfinite(o).all()
     assert rel(o.permute(0, 2, 1, 3), ref) < 2e-3
