@@ -347,6 +347,14 @@ __global__ void store_hidden_kernel(const float* __restrict__ x, const int* __re
     hidden[((long long)b * max_rows + row) * D + i] = x[(long long)b * D + i];
 }
 
+// torch.argmax order: a NaN ranks above every number, then the larger value, then the lower index wins.  So a row with NaN logits gives
+// the id HF greedy search gives, and an all-NaN row gives id 0 instead of no id at all.
+SEEDX_DEVINL bool argmax_before(float v, int i, float best, int bi) {
+  const bool vn = isnan(v), bn = isnan(best);
+  if (vn != bn) return vn;
+  return v > best || ((v == best || vn) && i < bi);
+}
+
 // logits processor (generation.py:19-31) + greedy argmax + sequence append, all on the device.
 // state[0] = sequence length, state[1] = done flag (EOS seen), state[2] = number of generated tokens
 __global__ void __launch_bounds__(1024)
@@ -377,13 +385,13 @@ logits_argmax_kernel(float* __restrict__ logits_all, int V, const int* __restric
     int bi = 0x7fffffff;
     for (int i = threadIdx.x; i < V; i += blockDim.x) {
       const float v = logits[i];
-      if (v > best || (v == best && i < bi)) best = v, bi = i;
+      if (argmax_before(v, i, best, bi)) best = v, bi = i;
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
       const float ov = __shfl_xor_sync(0xffffffffu, best, o);
       const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-      if (ov > best || (ov == best && oi < bi)) best = ov, bi = oi;
+      if (argmax_before(ov, oi, best, bi)) best = ov, bi = oi;
     }
     if ((threadIdx.x & 31) == 0) smax[threadIdx.x >> 5] = best, sidx[threadIdx.x >> 5] = bi;
     __syncthreads();
@@ -394,7 +402,7 @@ logits_argmax_kernel(float* __restrict__ logits_all, int V, const int* __restric
       for (int o = 16; o > 0; o >>= 1) {
         const float ov = __shfl_xor_sync(0xffffffffu, best, o);
         const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-        if (ov > best || (ov == best && oi < bi)) best = ov, bi = oi;
+        if (argmax_before(ov, oi, best, bi)) best = ov, bi = oi;
       }
       if (threadIdx.x == 0) sidx[0] = bi;
     }

@@ -30,7 +30,7 @@ def unary_f16(x, out=None, act=ACT_NONE):
 
 
 def scatter_rows(src, idx, dst, src_idx=None):
-    rows = src if src_idx is None else src[src_idx.long()]
+    rows = src[: idx.numel()] if src_idx is None else src[src_idx.long()]       # without src_idx, row r of src goes to idx[r]
     dst[idx.long()] = rows.float()
     return dst
 
@@ -122,7 +122,7 @@ def layernorm(x, gamma, beta, eps, out=None, *, out_dtype=torch.float16, rms=Fal
         out = torch.empty(x2.shape, dtype=out_dtype)
     out.reshape(-1, x2.shape[-1]).copy_(y.to(out.dtype))
     if add is not None:                                          # second output y + add[row % add_rows]
-        y2 = y + add.repeat(x2.shape[0] // add.shape[0], 1)
+        y2 = y + add.repeat(-(-x2.shape[0] // add.shape[0]), 1)[: x2.shape[0]]
         out2 = torch.empty(x2.shape, dtype=out.dtype) if out2 is None else out2
         out2.copy_(y2.to(out2.dtype))
         return out, out2

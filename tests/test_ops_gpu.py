@@ -2,6 +2,7 @@
 import pytest
 import torch
 import torch.nn.functional as F
+from fp16_ulp import ulp16
 
 pytestmark = pytest.mark.gpu
 
@@ -97,7 +98,22 @@ def test_attention_strided_qkv():
     assert rel(o.permute(0, 2, 1, 3), ref) < 2e-3
 
 
-@pytest.mark.parametrize("rows,cols", [(2048, 1664), (5, 208), (300, 4096), (174, 5120), (64, 1024), (7, 8192)])
+# seedx_layernorm picks its kernel from the shape (norm.cu, LN_VEC_DISPATCH): rows >= 64 and cols <= 2048 -> the warp-persistent rows kernel
+# (NV 4/8/12/16 for cols <= 512/1024/1536/2048); otherwise one warp per row (TPR 32, NV 2/4/8/16 for cols <= 256/512/1024/2048) or one CTA
+# per row (TPR 256, NV 4/8 for cols <= 4096/8192).  Unaligned rows or cols % 4 != 0 take the scalar kernel (test_layernorm_scalar_and_mixed_dtypes).
+@pytest.mark.parametrize("rows,cols", [
+    (2048, 1664),   # rows kernel, NV 16 (ViT width)
+    (5, 208),       # TPR 32, NV 2
+    (300, 4096),    # TPR 256, NV 4
+    (174, 5120),    # TPR 256, NV 8 (LLaMA prefill)
+    (64, 1024),     # rows kernel, NV 8
+    (7, 8192),      # TPR 256, NV 8 at the widest vectorised row
+    (128, 320),     # rows kernel, NV 4
+    (96, 1280),     # rows kernel, NV 12
+    (33, 320),      # TPR 32, NV 4
+    (7, 1024),      # TPR 32, NV 8
+    (8, 1664),      # TPR 32, NV 16
+])
 def test_layernorm_rmsnorm(rows, cols):
     from seedx_b200 import ops
     x = mk((rows, cols), 1, 3.0) + 0.5
@@ -112,6 +128,64 @@ def test_layernorm_rmsnorm(rows, cols):
         assert rel(y2, ref + add.repeat(rows // add.shape[0], 1)) < 1e-5
     rms = x * torch.rsqrt(x.pow(2).mean(-1, keepdim=True) + 1e-5) * g
     assert rel(ops.layernorm(x, g, None, 1e-5, out_dtype=torch.float32, rms=True), rms) < 1e-5
+
+
+def _ln64(x, g, eps, rms):
+    """float64 normalised row times gamma (the bias is added by the caller)"""
+    x = x.double()
+    if rms:
+        return x * torch.rsqrt(x.pow(2).mean(-1, keepdim=True) + eps) * g.double()
+    return (x - x.mean(-1, keepdim=True)) * torch.rsqrt(x.var(-1, unbiased=False, keepdim=True) + eps) * g.double()
+
+
+# fp32 outputs: max |y - ref| / max |ref|.  The statistics are fp32 sums over the row (two passes), rstd one rsqrtf, then (x - mean) rstd g + b
+# in fp32, so the error is a few fp32 ulps of the row's scale.
+LN_F32_TOL = 6e-7        # worst measured 1.6e-7 on an H100 80GB HBM3 (SXM, 700 W power limit)
+
+
+@pytest.mark.parametrize("rows,cols,tin,tout,pad,add_rows", [
+    (64, 1280, torch.float32, torch.float32, 2, 0),     # scalar: row stride 1282 floats is not a multiple of 4
+    (9, 640, torch.float16, torch.float16, 6, 4),       # scalar: row stride 646 halves, add_rows 4 does not divide 9
+    (70, 1001, torch.float16, torch.float16, 0, 64),    # scalar: cols % 4 != 0, add_rows 64 does not divide 70
+    (3, 1001, torch.float32, torch.float16, 0, 0),      # scalar, fp32 -> fp16
+    (5, 1001, torch.float16, torch.float32, 0, 2),      # scalar, fp16 -> fp32
+    (100, 1280, torch.float16, torch.float32, 0, 64),   # rows kernel NV 12, fp16 -> fp32, add_rows 64 does not divide 100
+    (200, 320, torch.float32, torch.float16, 0, 0),     # rows kernel NV 4, fp32 -> fp16
+    (10, 2048, torch.float32, torch.float16, 0, 4),     # TPR 32 NV 16, fp32 -> fp16, add_rows 4 does not divide 10
+    (6, 5120, torch.float16, torch.float32, 0, 4),      # TPR 256 NV 8 (LLaMA final norm), fp16 -> fp32, add_rows 4 does not divide 6
+])
+def test_layernorm_scalar_and_mixed_dtypes(rows, cols, tin, tout, pad, add_rows, record_property):
+    """LayerNorm and RMSNorm through the calls the shape-only cases above do not make: strided and unaligned rows, cols % 4 != 0, mixed input
+    and output dtypes, and the second output y + add[row % add_rows] with add_rows not dividing rows, all against float64.
+    fp16 outputs must be within 1 fp16 ulp of the float64 result: they are rounded once from an fp32 value within half an ulp plus its fp32
+    error, and that error, bounded here by (|x_hat g| + |b| + |add|) 2^-19, only matters where y cancels to within a few thousandths of 0."""
+    from seedx_b200 import ops
+    g = torch.Generator(device="cpu").manual_seed(rows * cols)
+    full = (torch.randn((rows, cols + pad), generator=g) * 3 + 0.5).to(tin)
+    x = full.cuda()[:, :cols]
+    gam, bet = torch.randn(cols, generator=g) + 1.0, torch.randn(cols, generator=g)
+    add = torch.randn((add_rows, cols), generator=g) if add_rows else None
+    worst_f32 = worst_ulps = 0.0
+    for rms in (False, True):
+        xg = _ln64(full[:, :cols], gam, 1e-6, rms)
+        b = torch.zeros(cols, dtype=torch.float64) if rms else bet.double()
+        refs = [(xg + b, xg.abs() + b.abs())]
+        if add_rows:
+            a = add.double().repeat(rows // add_rows + 1, 1)[:rows]
+            refs.append((xg + b + a, xg.abs() + b.abs() + a.abs()))
+        got = ops.layernorm(x, gam.cuda(), None if rms else bet.cuda(), 1e-6, out_dtype=tout, rms=rms, add=add.cuda() if add_rows else None)
+        for y, (r, mag) in zip(got if add_rows else (got,), refs):
+            assert y.dtype == tout
+            d = (y.cpu().double() - r).abs()
+            assert torch.isfinite(y).all()
+            if tout == torch.float16:
+                worst_ulps = max(worst_ulps, (d / ulp16(r)).max().item())
+                assert (d <= ulp16(r) + mag * 2.0 ** -19).all(), (d / ulp16(r)).max().item()
+            else:
+                worst_f32 = max(worst_f32, (d.max() / r.abs().max()).item())
+                assert (d <= LN_F32_TOL * r.abs().max()).all(), (d.max() / r.abs().max()).item()
+    record_property("fp16_out_ulps", worst_ulps)
+    record_property("fp32_out_err", worst_f32)
 
 
 @pytest.mark.parametrize("n,h,w,c1,c2,silu", [(2, 32, 32, 320, 0, True), (2, 16, 16, 1280, 640, True), (1, 64, 64, 640, 320, False),
