@@ -123,6 +123,9 @@ int seedx_gemm_set_workspace(void* device_buffer, int64_t bytes);
 void seedx_gemm_set_stream_k(int mode);
 /* A/B switch for the epilogue: 1 (default) = output/residual tiles staged in shared memory and moved by TMA, 0 = direct row-per-thread stores */
 void seedx_gemm_set_tma_epilogue(int on);
+/* what the most recent seedx_gemm_f16 launch ran, as decided on the host: out = {tile width, CTAs per cluster (1/2), stream-K (0/1),
+ * TMA epilogue (0/1), 16-byte vector stores allowed for the direct epilogue (0/1), pipeline stages}; all zero before the first launch */
+void seedx_gemm_last_config(int32_t out[6]);
 
 
 /* ------------------------------------------------------------------------------------------------

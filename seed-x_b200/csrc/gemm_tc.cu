@@ -744,6 +744,8 @@ static float* g_sk_scratch = nullptr;
 static size_t g_sk_scratch_bytes = 0;
 static unsigned* g_sk_flags = nullptr;
 constexpr size_t SK_FLAG_BYTES = 16384;
+// what the most recent launch ran (seedx_gemm_last_config): tile width, cluster size, stream-K, TMA epilogue, vec_ok, pipeline stages
+static int g_gemm_last[6] = {0, 0, 0, 0, 0, 0};
 
 template <int BN, int CL>
 static int launch_gemm_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& td, const CUtensorMap& tr, const GemmParams& p_in,
@@ -822,6 +824,7 @@ static int launch_gemm_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CU
   attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pdl_enabled() ? 2 : 1;
+  g_gemm_last[0] = BN, g_gemm_last[1] = CL, g_gemm_last[2] = p.stream_k, g_gemm_last[3] = p.tma_epi, g_gemm_last[4] = p.vec_ok, g_gemm_last[5] = p.stages;
   const cudaError_t e = (kHasSK && p.stream_k) ? cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, CL, kHasSK>, ta, tb, td, tr, p)
                                                : cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, CL, false>, ta, tb, td, tr, p);
   count_launch();
@@ -888,6 +891,9 @@ using namespace seedx;
 extern "C" void seedx_gemm_set_debug(void* device_buffer) { seedx::g_gemm_dbg = (unsigned long long*)device_buffer; }
 extern "C" void seedx_gemm_set_cluster(int mode) { seedx::g_gemm_cluster = mode; }
 extern "C" void seedx_gemm_set_tma_epilogue(int on) { seedx::g_gemm_tma_epi = on; }
+extern "C" void seedx_gemm_last_config(int32_t out[6]) {
+  for (int i = 0; i < 6; ++i) out[i] = seedx::g_gemm_last[i];
+}
 extern "C" void seedx_gemm_set_stream_k(int mode) {
   seedx::g_gemm_stream_k = mode;
   if (const char* e = getenv("SEEDX_SK_MIN_KBLOCKS")) seedx::g_sk_min_kblocks = atoi(e);
@@ -922,8 +928,10 @@ extern "C" int seedx_gemm_f16(const seedx_gemm_args* a, void* stream) {
   // ---- TMA epilogue eligibility (output / residual tiles go through shared memory and cp.async.bulk.tensor stores)
   const int out_es = a->out_dtype == SEEDX_F32 ? 4 : 2;
   const long long n_out_ll = a->gated ? a->N / 2 : a->N;
+  // The output rows must also END on a 16-byte boundary: on an H100 a TMA store box that straddles the end of a row writes the whole 16-byte
+  // granule, i.e. up to 14 bytes past n_out into the ldd gap of an output view (measured: 4 fp16 columns per row for n_out = 196).
   bool tma_epi = g_gemm_tma_epi && ((uintptr_t)a->D % 16 == 0) && ((a->ldd * out_es) % 16 == 0) && (a->batch == 1 || (a->strideD * out_es) % 16 == 0) &&
-                 (a->N % 2 == 0);
+                 (a->N % 2 == 0) && ((n_out_ll * out_es) % 16 == 0);
   if (a->residual) {
     tma_epi = tma_epi && !a->gated && a->residual_dtype == a->out_dtype && ((uintptr_t)a->residual % 16 == 0) && ((a->ldr * out_es) % 16 == 0) &&
               (a->res_row_mod % 32 == 0) && (a->batch == 1 || a->strideR == 0 || (a->strideR * out_es) % 16 == 0);

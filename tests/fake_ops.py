@@ -47,7 +47,7 @@ def gemm(a, w, out=None, *, bias=None, bias_m=None, bias_g=None, bias_g_rows=0, 
          out_dtype=torch.float16, ln=None, dynamic_b=False, row_part=None, col_part=None, row_stats=None, **kw):
     assert a.dtype == torch.float16 and w.dtype == torch.float16 and a.dim() == 2 and not any(v is not None and v is not False and v != 0 for v in kw.values())
     if residual is not None and res_row_mod:                     # residual row = output row % res_row_mod (position tables)
-        residual = residual.repeat(a.shape[0] // res_row_mod, 1)
+        residual = residual.repeat(-(-a.shape[0] // res_row_mod), 1)[: a.shape[0]]
     acc = alpha * (a.float() @ w.float().t())
     if ln is not None:                                           # folded LayerNorm: rstd * (acc - mean * colsum)
         st, cs = ln[0], ln[1]
@@ -61,10 +61,10 @@ def gemm(a, w, out=None, *, bias=None, bias_m=None, bias_g=None, bias_g_rows=0, 
     if bias_m is not None:                                       # one bias per output ROW (transposed products)
         acc = acc + bias_m[:, None]
     if bias_g is not None:                                       # one additive row per group of bias_g_rows output rows
-        acc = acc + bias_g.repeat_interleave(bias_g_rows, dim=0)
-    if gated:                                                    # interleaved rows [value_j, gate_j]
+        acc = acc + bias_g.repeat_interleave(bias_g_rows, dim=0)[: a.shape[0]]
+    if gated:                                                    # interleaved rows [value_j, gate_j]; ACT_NONE gates with the plain product
         g = acc[:, 1::2]
-        acc = acc[:, 0::2] * (F.silu(g) if act == ACT_SILU else F.gelu(g))
+        acc = acc[:, 0::2] * (F.silu(g) if act == ACT_SILU else F.gelu(g) if act == ACT_GELU else g)
     elif act == ACT_SILU:
         acc = F.silu(acc)
     elif act == ACT_GELU:
@@ -298,6 +298,8 @@ def conv2d_nhwc(x, w, out=None, *, taps=3, bias=None, bias_g=None, residual=None
     y = y.permute(0, 2, 3, 1)
     if act == ACT_SILU:
         y = F.silu(y)
+    elif act == ACT_GELU:
+        y = F.gelu(y)
     if residual is not None:
         y = y + residual.float()
     if out is None:

@@ -3,6 +3,8 @@ declares; the product path refuses to run without CUDA (no CPU fallback); host-s
 import ctypes
 import os
 import re
+import subprocess
+import sys
 
 import pytest
 import torch
@@ -24,7 +26,13 @@ def test_library_exports_every_declared_symbol():
     missing = [n for n in names if not hasattr(lib, n)]
     assert not missing, missing
     assert _lib.lib().seedx_abi_version() == 2
-    assert _lib.launch_count() == 0          # nothing has been launched: importing / loading does not touch a device
+    # nothing is launched by importing / loading the library: checked in a fresh interpreter, so that GPU tests run earlier in this process
+    # (whose launches the counter rightly includes) do not matter
+    probe = "import sys; sys.path.insert(0, sys.argv[1]); from seedx_b200 import _lib; _lib.lib(); print(_lib.launch_count())"
+    flags = ["-s"] if sys.flags.no_user_site else []
+    r = subprocess.run([sys.executable, *flags, "-c", probe, ROOT], capture_output=True, text=True, cwd=ROOT)
+    assert r.returncode == 0, r.stderr
+    assert r.stdout.strip() == "0", r.stdout
 
 
 def test_no_cpu_fallback():

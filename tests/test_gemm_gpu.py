@@ -232,23 +232,67 @@ def stream_k_mode(request):
     lib().seedx_gemm_set_stream_k(1)
 
 
-@pytest.mark.parametrize("M,N,K,tile_n", [(8192, 1280, 1280, 0), (8192, 1280, 5120, 224), (8192, 1280, 320, 256), (32768, 640, 640, 0), (4096, 3072, 1024, 160),
-                                          (2500, 1000, 4096, 128), (19000, 520, 192, 64), (8192, 10240, 1280, 0)])
-def test_gemm_stream_k(M, N, K, tile_n, stream_k_mode, cluster_mode):
+def last_config():
+    """what the last seedx_gemm_f16 launch ran (seedx_gemm_last_config)"""
+    import ctypes
+    from seedx_b200._lib import lib
+    v = (ctypes.c_int32 * 6)()
+    lib().seedx_gemm_last_config(v)
+    return dict(zip(("tile", "cluster", "stream_k", "tma", "vec", "stages"), list(v)))
+
+
+def stream_k_legal(cfg, M, N, k_blocks):
+    """True where the forced stream-K schedule must run: a cluster-pair kernel with stream-K variants (width >= 128, multiple of 32) and more
+    pair tiles than an H100 has cluster pairs, so every cluster starts inside a tile"""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    groups = (-(-M // 128) + 1) // 2 * -(-N // cfg["tile"])
+    return cfg["cluster"] == 2 and cfg["tile"] % 32 == 0 and cfg["tile"] >= 128 and groups > sms // 2 and groups * k_blocks >= 4 * (sms // 2)
+
+
+# (M, N, K, tile_n) x schedule.  Single-CTA tiles and 64-wide tiles have no stream-K kernel, so the stream-K schedule is only paired with
+# cluster pairs; the ids keep the form [schedule-cluster-M-N-K-tile_n].
+_SK_SHAPES = [(8192, 1280, 1280, 0), (8192, 1280, 5120, 224), (8192, 1280, 320, 256), (32768, 640, 640, 0), (4096, 3072, 1024, 160),
+              (2500, 1000, 4096, 128), (8192, 10240, 1280, 0),
+              (6000, 1000, 1032, 192),   # ragged M (47 m-blocks: the last pair's second CTA past M), ragged N and K
+              (4000, 1256, 520, 256),    # 80 pair tiles: just more than the cluster pairs of an H100
+              (5000, 904, 2056, 160),    # ragged last tile (104 of 160 columns), K = 32 k-blocks + 8
+              (2900, 3000, 600, 128)]    # one partial m-block, 24 column blocks
+_SK_CASES = [pytest.param(M, N, K, t, sk, cl, id=f"{sk}-{cl}-{M}-{N}-{K}-{t}")
+             for sk, cl in (("data_parallel", "single_cta"), ("data_parallel", "cluster2"), ("stream_k", "cluster2")) for M, N, K, t in _SK_SHAPES]
+
+
+@pytest.mark.parametrize("M,N,K,tile_n,schedule,cluster", _SK_CASES)
+def test_gemm_stream_k(M, N, K, tile_n, schedule, cluster):
     """stream-K: clusters take equal shares of the (tile, k-block) iterations; tiles cut between clusters are completed through the fp32 partial
     workspace in a fixed order.  Same results as the data-parallel schedule to fp32 summation order, bit-identical from run to run, with every
-    epilogue kind (bias, gating, in-place residual through the TMA epilogue, fp32 output)."""
+    epilogue kind (bias, gating, in-place residual through the TMA epilogue, fp32 output).  seedx_gemm_last_config confirms the schedule ran."""
+    from seedx_b200._lib import lib
+    lib().seedx_gemm_set_cluster(0 if cluster == "single_cta" else 2)
+    lib().seedx_gemm_set_stream_k(0 if schedule == "data_parallel" else 2)
+    try:
+        _gemm_stream_k(M, N, K, tile_n, schedule)
+    finally:
+        lib().seedx_gemm_set_cluster(1)
+        lib().seedx_gemm_set_stream_k(1)
+
+
+def _gemm_stream_k(M, N, K, tile_n, schedule):
     from seedx_b200 import ops
     a = mk((M, K), 71).half()
     w = mk((N, K), 72, K ** -0.5).half()
     bias = mk((N,), 73)
     acc = a.float() @ w.float().t() + bias
     o32 = ops.gemm(a, w, bias=bias, out_dtype=torch.float32, tile_n=tile_n)
+    cfg = last_config()
+    if schedule == "stream_k":
+        assert stream_k_legal(cfg, M, N, -(-K // 64)), cfg
+    assert cfg["stream_k"] == (schedule == "stream_k"), cfg
     assert rel(o32, acc) < 1e-5
     assert torch.equal(o32, ops.gemm(a, w, bias=bias, out_dtype=torch.float32, tile_n=tile_n))
     r = mk((M, N), 74).half()
     want = acc + r.float()
     ops.gemm(a, w, out=r, bias=bias, residual=r, tile_n=tile_n)
+    assert last_config()["stream_k"] == (schedule == "stream_k")
     assert rel(r, want) < 2e-3
     if N % 2 == 0:
         o = ops.gemm(a, w, bias=bias, act=ops.ACT_GELU, gated=True, tile_n=tile_n)
@@ -257,6 +301,17 @@ def test_gemm_stream_k(M, N, K, tile_n, stream_k_mode, cluster_mode):
 
 @pytest.mark.parametrize("n,h,w,c,cout", [(8, 32, 32, 1280, 1280), (2, 64, 64, 640, 640), (3, 32, 32, 320, 640)])
 def test_conv_stream_k(n, h, w, c, cout, stream_k_mode):
+    """3x3 convs with per-image bias, fp16 residual and column statistics, in cluster pairs (the only kernels with a stream-K variant);
+    seedx_gemm_last_config confirms the schedule wherever it is legal"""
+    from seedx_b200._lib import lib
+    lib().seedx_gemm_set_cluster(2)
+    try:
+        _conv_stream_k(n, h, w, c, cout, stream_k_mode)
+    finally:
+        lib().seedx_gemm_set_cluster(1)
+
+
+def _conv_stream_k(n, h, w, c, cout, stream_k_mode):
     from seedx_b200 import ops
     x = mk((n, c, h, w), 81).half()
     wt = mk((cout, c, 3, 3), 82, (c * 9) ** -0.5).half()
@@ -267,6 +322,12 @@ def test_conv_stream_k(n, h, w, c, cout, stream_k_mode):
     res = mk((n, h, w, cout), 85).half()
     part = torch.empty((n * h * w // 32, cout, 2), device="cuda")
     o = ops.conv2d_nhwc(xn, wp, taps=3, bias=bias, bias_g=temb, residual=res, col_part=part)
+    cfg = last_config()
+    assert cfg["cluster"] == 2
+    if stream_k_mode == "data_parallel":
+        assert cfg["stream_k"] == 0
+    elif stream_k_legal(cfg, n * h * w, cout, 9 * c // 64):
+        assert cfg["stream_k"] == 1, cfg
     assert rel(o, ref + res.float()) < 2e-3
     c32 = o.float().view(-1, 32, cout)
     assert rel(part[..., 0], c32.sum(1)) < 1e-5
