@@ -234,6 +234,15 @@ int seedx_cfg_euler_step(const float* eps, float* x, void* unet_in, int64_t batc
  * replaces the M=1 projections of modeling_llama_xformer.py:204-206,239,166-167,707 (+ LlamaRMSNorm :258-259,443) */
 int seedx_gemv_f16(const void* W, const float* x, int64_t ldx, const float* rms_w, float eps, const float* residual, int64_t ldr, float* out,
                    int64_t ldo, int64_t N, int64_t K, int batch, int gated, void* stream);
+/* the same GEMV over FP8 weights: W8 = e4m3 (OCP "fn" variant) [N, K] row-major, 16B aligned, K % 64 == 0; row_scale fp32 [N], weight
+ * row n = row_scale[n] * W8[n, :].  The scale multiplies the fp32 dot product: out[b][n] = s[n] * dot(n, b) (+ residual[b][n]); gated (rows
+ * interleaved [up_j, gate_j]): out[b][j] = s[2j] * up * silu(s[2j+1] * gate).  Half the weight bytes of seedx_gemv_f16 per token. */
+int seedx_gemv_fp8(const void* W8, const float* row_scale, const float* x, int64_t ldx, const float* rms_w, float eps, const float* residual,
+                   int64_t ldr, float* out, int64_t ldo, int64_t N, int64_t K, int batch, int gated, void* stream);
+/* fp16 out[n, k] = (half)(float(W8[n, k]) * row_scale[n]) for an FP8 weight [N, K] (K % 16 == 0, W8 and out 16B aligned): feeds the prefill
+ * GEMM of an FP8 model.  Its stores wait for the preceding kernel (PDL), so out may be a scratch buffer that kernel still reads; the GEMM that
+ * reads out must treat it as a dynamic operand (seedx_gemm_args.b_dynamic = 1). */
+int seedx_dequant_fp8(const void* W8, const float* row_scale, void* out, int64_t N, int64_t K, void* stream);
 /* one new token per sequence: RoPE(q,k) (:141-149), append k,v at position state[b][0]-1 (replaces torch.cat :215-218), attention
  * over the cache (:225-237).  qkv fp32 [batch][3*H*d]; caches fp16 [batch][max_len, H*d] (cache_stride elements apart); out fp32 [batch][H*d] */
 int seedx_decode_attention(const float* qkv, const int32_t* state, const float* inv_freq, void* kcache, void* vcache, int64_t cache_stride,

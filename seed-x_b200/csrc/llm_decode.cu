@@ -149,6 +149,164 @@ gemv_mma_kernel(const __half* __restrict__ W, const float* __restrict__ x, long 
 }
 
 // ------------------------------------------------------------------------------------------------
+// FP8 (e4m3) weights: the same GEMV with half the bytes per row.  W8 holds q[n,k] and row_scale s[n] (fp32) such that the weight is
+// s[n] * q[n,k]; the scale is applied to the fp32 dot product in the epilogue.  A lane's 16-byte load now carries 16 consecutive e4m3
+// weights of its row, k = kb*64 + q*16 .. +15; cvt.rn.f16x2.e4m3x2 turns them into 8 f16x2 registers (exactly: every e4m3 value is an
+// fp16 value) that feed four m16n8k16 MMAs.  As in gemv_mma_kernel, lane (g, q) supplies k-slots {2q,2q+1,2q+8,2q+9} for the weights of
+// row g AND for the activations of sequence g, so reading the activations at the same 16 k positions keeps the pairing right.
+// Same register budget as the fp16 kernel: GEMV8_MAXKB x 16 B of weights per lane, which covers K = 13824 in one unit.
+// ------------------------------------------------------------------------------------------------
+constexpr int GEMV8_MAXKB = 14;  // 64-wide k blocks a warp keeps in registers (16 B per lane each)
+
+SEEDX_DEVINL uint32_t e4m3x2_to_f16x2(uint16_t v) {   // low byte -> low half (the lower k), high byte -> high half
+  uint32_t r;
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;\n" : "=r"(r) : "h"(v));
+  return r;
+}
+
+template <int NB>  // sequence slots held in shared memory: 1, 2, 4 or 8
+__global__ void __launch_bounds__(GEMV_THREADS, 1)
+gemv_fp8_kernel(const uint8_t* __restrict__ W8, const float* __restrict__ row_scale, const float* __restrict__ x, long long ldx,
+                const float* __restrict__ rms_w, float eps, const float* __restrict__ residual, long long ldr, float* __restrict__ out,
+                long long ldo, int N, int K, int gated) {
+  extern __shared__ __align__(16) uint8_t gsm[];
+  __half* xs = (__half*)gsm;                                   // [NB][K + 8]: rows 16 B apart in bank space (conflict-free LDS.128)
+  const int KP = K + 8;
+  __shared__ float part_sm[2][GEMV_WARPS][GEMV_ROWS * 8];
+  __shared__ float red[GEMV_WARPS][NB];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+  const int g = lane >> 2, q = lane & 3;   // g: weight row inside the tile AND sequence slot of the B fragment; q: 16-byte k-chunk
+  const int tiles = (N + GEMV_ROWS - 1) / GEMV_ROWS;
+  const int t_begin = (int)((long long)blockIdx.x * tiles / gridDim.x);
+  const int t_end = (int)((long long)(blockIdx.x + 1) * tiles / gridDim.x);
+  const int kblocks = K >> 6;              // 64-wide k blocks (K % 64 == 0 checked on the host)
+  const int kb_begin = (int)((long long)warp * kblocks / GEMV_WARPS), kb_end = (int)((long long)(warp + 1) * kblocks / GEMV_WARPS);
+  const int kparts = (((kblocks + GEMV_WARPS - 1) / GEMV_WARPS) + GEMV8_MAXKB - 1) / GEMV8_MAXKB;   // block-uniform
+  const bool has_x = g < NB;
+
+  // software pipeline across tiles, as in gemv_mma_kernel: unit u+1 is requested before the cross-warp reduction of unit u
+  uint4 wreg[GEMV8_MAXKB];
+  auto load_unit = [&](int t, int part) {
+    const int row = min(t * GEMV_ROWS + g, N - 1);
+    const uint4* wrow = (const uint4*)(W8 + (long long)row * K) + q;
+    const int kb0 = kb_begin + part * GEMV8_MAXKB;
+#pragma unroll
+    for (int i = 0; i < GEMV8_MAXKB; ++i)
+      if (kb0 + i < kb_end) wreg[i] = __ldcs(wrow + (kb0 + i) * 4);   // 16 consecutive e4m3 of weight row g: k = kb*64 + q*16 ..
+  };
+  if (t_begin < t_end) load_unit(t_begin, 0);   // weights never depend on the previous kernel: requested before the PDL wait
+  pdl_wait();
+  pdl_trigger();
+  // ---- prologue: activations -> (RMSNorm) -> fp16 in shared memory
+  float ss[NB];
+#pragma unroll
+  for (int b = 0; b < NB; ++b) ss[b] = 0.f;
+  if (rms_w != nullptr) {
+    for (int k = threadIdx.x; k < K; k += GEMV_THREADS) {
+#pragma unroll
+      for (int b = 0; b < NB; ++b) {
+        const float v = x[b * ldx + k];
+        ss[b] += v * v;
+      }
+    }
+#pragma unroll
+    for (int b = 0; b < NB; ++b) {
+      ss[b] = warp_sum(ss[b]);
+      if (lane == 0) red[warp][b] = ss[b];
+    }
+    __syncthreads();
+#pragma unroll
+    for (int b = 0; b < NB; ++b) {
+      float t = 0.f;
+#pragma unroll
+      for (int w = 0; w < GEMV_WARPS; ++w) t += red[w][b];
+      ss[b] = rsqrtf(t / (float)K + eps);
+    }
+  }
+  for (int k = threadIdx.x; k < K; k += GEMV_THREADS) {
+    const float g = rms_w ? rms_w[k] : 1.f;
+#pragma unroll
+    for (int b = 0; b < NB; ++b) {
+      const float v = x[b * ldx + k];
+      xs[b * KP + k] = __float2half_rn(rms_w ? v * ss[b] * g : v);
+    }
+  }
+  __syncthreads();
+
+  const __half* xrow = xs + (has_x ? g : 0) * KP + q * 16;
+  int buf = 0;
+  for (int t = t_begin; t < t_end; ++t, buf ^= 1) {
+    float c[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int part = 0; part < kparts; ++part) {
+      const int kb0 = kb_begin + part * GEMV8_MAXKB;
+#pragma unroll
+      for (int i = 0; i < GEMV8_MAXKB; ++i) {
+        if (kb0 + i < kb_end) {
+          uint4 x0 = make_uint4(0, 0, 0, 0), x1 = make_uint4(0, 0, 0, 0);
+          if (has_x) {                                                   // the same 16 k positions of sequence g
+            x0 = *(const uint4*)(xrow + (kb0 + i) * 64);
+            x1 = *(const uint4*)(xrow + (kb0 + i) * 64 + 8);
+          }
+          const uint4 w = wreg[i];
+          mma16816_f32(c, e4m3x2_to_f16x2((uint16_t)w.x), 0u, e4m3x2_to_f16x2((uint16_t)(w.x >> 16)), 0u, x0.x, x0.y);
+          mma16816_f32(c, e4m3x2_to_f16x2((uint16_t)w.y), 0u, e4m3x2_to_f16x2((uint16_t)(w.y >> 16)), 0u, x0.z, x0.w);
+          mma16816_f32(c, e4m3x2_to_f16x2((uint16_t)w.z), 0u, e4m3x2_to_f16x2((uint16_t)(w.z >> 16)), 0u, x1.x, x1.y);
+          mma16816_f32(c, e4m3x2_to_f16x2((uint16_t)w.w), 0u, e4m3x2_to_f16x2((uint16_t)(w.w >> 16)), 0u, x1.z, x1.w);
+        }
+      }
+      if (part + 1 < kparts) load_unit(t, part + 1);
+      else if (t + 1 < t_end) load_unit(t + 1, 0);
+    }
+    part_sm[buf][warp][g * 8 + 2 * q] = c[0];
+    part_sm[buf][warp][g * 8 + 2 * q + 1] = c[1];
+    __syncthreads();
+    if (threadIdx.x < GEMV_ROWS * NB) {
+      const int r = threadIdx.x / NB, b = threadIdx.x % NB;
+      float v = 0.f;
+#pragma unroll
+      for (int w = 0; w < GEMV_WARPS; ++w) v += part_sm[buf][w][r * 8 + b];
+      const int orow = t * GEMV_ROWS + r;
+      if (!gated) {
+        if (orow < N) out[b * ldo + orow] = row_scale[orow] * v + (residual ? residual[b * ldr + orow] : 0.f);
+      } else if ((r & 1) == 0 && orow + 1 < N) {
+        float gate = 0.f;
+#pragma unroll
+        for (int w = 0; w < GEMV_WARPS; ++w) gate += part_sm[buf][w][(r + 1) * 8 + b];
+        out[b * ldo + (orow >> 1)] = (row_scale[orow] * v) * silu(row_scale[orow + 1] * gate);   // rows [up_j, gate_j], each with its scale
+      }
+    }
+  }
+}
+
+// out[n, k] = (half)(float(q[n, k]) * s[n]): one 16-byte load of 16 e4m3 values, two 16-byte stores of fp16.  The output is a scratch
+// buffer that the kernels before this one may still read, so every store waits for the PDL dependency; the loads do not.
+__global__ void __launch_bounds__(256)
+dequant_fp8_kernel(const uint4* __restrict__ q, const float* __restrict__ row_scale, uint4* __restrict__ out, long long chunks, int row_chunks) {
+  long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  uint4 w = make_uint4(0, 0, 0, 0);
+  if (i < chunks) w = __ldcs(q + i);
+  pdl_wait();
+  pdl_trigger();
+  for (; i < chunks; i += (long long)gridDim.x * blockDim.x) {
+    const float s = __ldg(row_scale + i / row_chunks);
+    const uint32_t wv[4] = {w.x, w.y, w.z, w.w};
+    uint32_t o[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const uint32_t h2 = e4m3x2_to_f16x2((uint16_t)(wv[j >> 1] >> ((j & 1) * 16)));
+      const float2 f = __half22float2(*(const __half2*)&h2);
+      const __half2 r = __floats2half2_rn(f.x * s, f.y * s);
+      o[j] = *(const uint32_t*)&r;
+    }
+    out[2 * i] = make_uint4(o[0], o[1], o[2], o[3]);
+    out[2 * i + 1] = make_uint4(o[4], o[5], o[6], o[7]);
+    const long long nx = i + (long long)gridDim.x * blockDim.x;
+    if (nx < chunks) w = __ldcs(q + nx);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // decode attention for one new token: RoPE(q,k) -> append k,v to the cache -> softmax(q K^T) V over positions 0..pos
 // one CTA per head, head_dim 128, 8 warps, each half-warp walks keys with 16-byte loads.
 // state[0] = current sequence length (the token being consumed sits at position state[0] - 1)
@@ -460,6 +618,50 @@ extern "C" int seedx_gemv_f16(const void* W, const float* x, int64_t ldx, const 
 #undef GEMV_LAUNCH
   count_launch();
   return check_cuda(cudaGetLastError(), "gemv launch");
+}
+
+extern "C" int seedx_gemv_fp8(const void* W8, const float* row_scale, const float* x, int64_t ldx, const float* rms_w, float eps,
+                              const float* residual, int64_t ldr, float* out, int64_t ldo, int64_t N, int64_t K, int batch, int gated, void* stream) {
+  SEEDX_REQUIRE(W8 && row_scale && x && out, "seedx_gemv_fp8: null pointer");
+  SEEDX_REQUIRE(batch >= 1 && batch <= 8, "seedx_gemv_fp8: batch %d out of range (1..8)", batch);
+  SEEDX_REQUIRE(K % 64 == 0 && K > 0 && N > 0, "seedx_gemv_fp8: K=%lld must be a positive multiple of 64", (long long)K);
+  SEEDX_REQUIRE((uintptr_t)W8 % 16 == 0, "seedx_gemv_fp8: W8 must be 16B aligned");
+  if (gated) SEEDX_REQUIRE(N % 2 == 0 && residual == nullptr, "seedx_gemv_fp8: gated needs even N and no residual");
+  const int nb = batch <= 1 ? 1 : batch <= 2 ? 2 : batch <= 4 ? 4 : 8;
+  SEEDX_REQUIRE(nb == batch, "seedx_gemv_fp8: batch must be 1, 2, 4 or 8 (pad the sequence slots)");
+  const size_t smem = (size_t)nb * (K + 8) * 2;
+  SEEDX_REQUIRE(smem <= 216 * 1024, "seedx_gemv_fp8: batch*K = %d*%lld does not fit in shared memory", nb, (long long)K);
+  const long long tiles = (N + GEMV_ROWS - 1) / GEMV_ROWS;
+  long long blocks = num_sms();
+  if (blocks > tiles) blocks = tiles;
+  cudaStream_t st = (cudaStream_t)stream;
+#define GEMV8_LAUNCH(NBV)                                                                                                              \
+  do {                                                                                                                                 \
+    static bool attr = false;                                                                                                          \
+    if (!attr) {                                                                                                                       \
+      SEEDX_CUDA(cudaFuncSetAttribute(gemv_fp8_kernel<NBV>, cudaFuncAttributeMaxDynamicSharedMemorySize, 216 * 1024));                 \
+      attr = true;                                                                                                                     \
+    }                                                                                                                                  \
+    launch_k(gemv_fp8_kernel<NBV>, (unsigned)blocks, GEMV_THREADS, smem, st, (const uint8_t*)W8, row_scale, x, ldx, rms_w, eps, residual, \
+             ldr, out, ldo, (int)N, (int)K, gated);                                                                                    \
+  } while (0)
+  if (nb == 1) GEMV8_LAUNCH(1);
+  else if (nb == 2) GEMV8_LAUNCH(2);
+  else if (nb == 4) GEMV8_LAUNCH(4);
+  else GEMV8_LAUNCH(8);
+#undef GEMV8_LAUNCH
+  count_launch();
+  return check_cuda(cudaGetLastError(), "gemv_fp8 launch");
+}
+
+extern "C" int seedx_dequant_fp8(const void* W8, const float* row_scale, void* out, int64_t N, int64_t K, void* stream) {
+  SEEDX_REQUIRE(W8 && row_scale && out, "seedx_dequant_fp8: null pointer");
+  SEEDX_REQUIRE(N > 0 && K > 0 && K % 16 == 0, "seedx_dequant_fp8: K=%lld must be a positive multiple of 16", (long long)K);
+  SEEDX_REQUIRE((uintptr_t)W8 % 16 == 0 && (uintptr_t)out % 16 == 0, "seedx_dequant_fp8: W8 and out must be 16B aligned");
+  const long long chunks = N * (K / 16);
+  launch_k(dequant_fp8_kernel, ew_grid(chunks, 256), 256, 0, (cudaStream_t)stream, (const uint4*)W8, row_scale, (uint4*)out, chunks, (int)(K / 16));
+  count_launch();
+  return check_cuda(cudaGetLastError(), "dequant_fp8 launch");
 }
 
 extern "C" int seedx_decode_attention(const float* qkv, const int32_t* state, const float* inv_freq, void* kcache, void* vcache,

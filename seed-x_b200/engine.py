@@ -21,9 +21,10 @@ VIT_G = dict(width=1664, layers=48, heads=16, mlp_width=8192, output_dim=4096, n
 
 class SeedXEngine:
     def __init__(self, vit_cfg=None, llm_cfg=None, unet_cfg=None, vae_cfg=None, rxl_cfg=None, device_weights=True, vit_sd=None,
-                 max_len=1024, log=None, edit=False):
+                 max_len=1024, log=None, edit=False, llm_weight_format="fp16"):
         """edit=True builds the SEED-X-Edit pipe (eval_img2edit_seed_x_edit.py): 8-channel conv_in UNet behind SDXLAdapterWithLatentImage and
-        the VAE encoder for the source image."""
+        the VAE encoder for the source image.  llm_weight_format: "fp16" or "fp8_e4m3" (LlamaForCausalLM's weight_format: FP8 projection
+        weights with per-row scales, half the bytes per decode step)."""
         log = log or (lambda *a: None)
         t0 = time.time()
         vit_cfg = dict(VIT_G if vit_cfg is None else vit_cfg)
@@ -49,7 +50,7 @@ class SeedXEngine:
             self.vit.load_state_dict(vit_sd)
             del vit_sd
             log(f"vit ready {time.time() - t0:.1f}s")
-            self.llm = LlamaForCausalLM(llm_cfg, max_len=max_len)
+            self.llm = LlamaForCausalLM(llm_cfg, max_len=max_len, weight_format=llm_weight_format)
             self.llm.load_state_dict(synth.llama_state_dict(llm_cfg))
             log(f"llm ready {time.time() - t0:.1f}s")
             D, V = llm_cfg["hidden"], vit_cfg["output_dim"]

@@ -17,6 +17,20 @@ from . import _lib, ops, trace
 from ._lib import SeedxError
 
 LLAMA_13B = dict(vocab=32330, hidden=5120, layers=40, heads=40, ffn=13824, eps=1e-5)
+WEIGHT_FORMATS = ("fp16", "fp8_e4m3")
+FP8_MAX = 448.0                                # largest finite float8_e4m3fn
+PROJECTIONS = ("wqkv", "wo", "wgu", "wdown")   # the packed per-layer matrices that weight_format="fp8_e4m3" stores in FP8
+
+
+def quantize_fp8_rows(w):
+    """Per-output-row FP8 quantisation of a weight [N, K]: s[n] = amax|w[n]| / 448 (1 for an all-zero row), q = w / s in float8_e4m3fn.
+    Returns (q, s fp32 [N]) with w[n] ~= s[n] * q[n].  The clamp matters: torch's cast turns anything beyond +-448 into NaN, and w / s can
+    round a hair above 448 at the row maximum."""
+    w = w.float()
+    s = w.abs().amax(dim=1) / FP8_MAX
+    s = torch.where(s > 0, s, torch.ones_like(s))
+    q = (w / s[:, None]).clamp(-FP8_MAX, FP8_MAX).to(torch.float8_e4m3fn)
+    return q.contiguous(), s.contiguous()
 
 
 class _Embedding:
@@ -94,7 +108,13 @@ class GreedySearchOutput(dict):
 
 
 class LlamaForCausalLM:
-    def __init__(self, cfg=None, max_len=2048, device="cuda", kv_page_size=64, kv_pages=None):
+    def __init__(self, cfg=None, max_len=2048, device="cuda", kv_page_size=64, kv_pages=None, weight_format="fp16"):
+        """weight_format="fp8_e4m3" stores the four projection matrices of every layer (wqkv, wo, wgu, wdown) as float8_e4m3fn with one
+        fp32 scale per output row: the token loop streams half the bytes (seedx_gemv_fp8) and prefill dequantizes each matrix into an fp16
+        scratch buffer right before its GEMM.  The embedding table, lm_head and the norms stay in fp16 / fp32."""
+        if weight_format not in WEIGHT_FORMATS:
+            raise SeedxError(f"weight_format {weight_format!r}: expected one of {WEIGHT_FORMATS}")
+        self.weight_format = weight_format
         self.cfg = dict(LLAMA_13B if cfg is None else cfg)
         self.device = torch.device(device)
         self.max_len = max_len
@@ -111,12 +131,12 @@ class LlamaForCausalLM:
 
     # ---- reference-compatible plumbing --------------------------------------------------------------------------------
     @classmethod
-    def from_pretrained(cls, pretrained_model_name_or_path, low_cpu_mem_usage=True, torch_dtype=None, **kw):
+    def from_pretrained(cls, pretrained_model_name_or_path, low_cpu_mem_usage=True, torch_dtype=None, weight_format="fp16", **kw):
         d = pretrained_model_name_or_path
         c = json.load(open(os.path.join(d, "config.json")))
         cfg = dict(vocab=c["vocab_size"], hidden=c["hidden_size"], layers=c["num_hidden_layers"], heads=c["num_attention_heads"],
                    ffn=c["intermediate_size"], eps=c.get("rms_norm_eps", 1e-5), eos=c.get("eos_token_id", 2))
-        m = cls(cfg)
+        m = cls(cfg, weight_format=weight_format)
         sd = {}
         idx = os.path.join(d, "pytorch_model.bin.index.json")
         sidx = os.path.join(d, "model.safetensors.index.json")
@@ -162,6 +182,13 @@ class LlamaForCausalLM:
                 wo=h(sd[p + "self_attn.o_proj.weight"]),
                 wgu=h(torch.stack([up, gate], dim=1).reshape(2 * up.shape[0], -1)),   # rows [up_0, gate_0, up_1, gate_1, ...]
                 wdown=h(sd[p + "mlp.down_proj.weight"])))
+            if self.weight_format == "fp8_e4m3":
+                L = self.layers[-1]
+                for k in PROJECTIONS:
+                    L[k], L[k + "_s"] = quantize_fp8_rows(L[k])
+        self._wscratch = None
+        if self.weight_format == "fp8_e4m3":   # prefill: each projection is dequantized here right before its GEMM (sized for the largest)
+            self._wscratch = torch.empty((max(L[k].numel() for L in self.layers for k in PROJECTIONS),), device=dev, dtype=torch.float16)
         self.norm = f(sd["model.norm.weight"])
         self.lm_head = h(sd["lm_head.weight"])
         if self.embed.shape[0] != cfg["vocab"] or self.lm_head.shape[0] != cfg["vocab"]:
@@ -213,13 +240,18 @@ class LlamaForCausalLM:
         dev, cfg = self.device, self.cfg
         D, Fh = cfg["hidden"], cfg["ffn"]
 
-        def fold(dst, name):
-            """dst: a (possibly strided) view into a packed fp16 weight; name: HF module name, e.g. model.layers.0.self_attn.q_proj"""
+        def fold(dst, name, scale=None):
+            """dst: a (possibly strided) view into a packed fp16 weight; name: HF module name, e.g. model.layers.0.self_attn.q_proj.
+            FP8 weights: dst is the float8_e4m3fn view and `scale` the matching rows of its scale vector; the rows are dequantized, updated
+            in fp32 and requantized, and both q and the scales are written in place."""
             w = plain.pop(name + ".weight", None)
             ab = lora.pop(name, None)
             if w is None and ab is None:
                 return
-            cur = w.to(dev).float() if w is not None else dst.float()
+            if w is not None:
+                cur = w.to(dev).float()
+            else:
+                cur = dst.float() * scale[:, None] if scale is not None else dst.float()
             if tuple(cur.shape) != tuple(dst.shape):
                 raise SeedxError(f"{name}.weight: shape {tuple(cur.shape)} != {tuple(dst.shape)}")
             if ab is not None:
@@ -227,7 +259,12 @@ class LlamaForCausalLM:
                 if tuple(delta.shape) != tuple(dst.shape):
                     raise SeedxError(f"LoRA update of {name}: shape {tuple(delta.shape)} != {tuple(dst.shape)}")
                 cur = cur + delta
-            dst.copy_(cur.to(torch.float16))
+            if scale is None:
+                dst.copy_(cur.to(torch.float16))
+            else:
+                q, sc = quantize_fp8_rows(cur)
+                dst.copy_(q)
+                scale.copy_(sc)
 
         def setf(dst, name):
             v = plain.pop(name, None)
@@ -238,13 +275,15 @@ class LlamaForCausalLM:
 
         for i, L in enumerate(self.layers):
             p = f"model.layers.{i}."
+            sq, so, sgu, sdown = (L.get(k + "_s") for k in PROJECTIONS)      # row scales of an FP8 model (None for fp16): sliced like the rows
             for j, n in enumerate(("q_proj", "k_proj", "v_proj")):
-                fold(L["wqkv"][j * D:(j + 1) * D], p + "self_attn." + n)
-            fold(L["wo"], p + "self_attn.o_proj")
+                fold(L["wqkv"][j * D:(j + 1) * D], p + "self_attn." + n, None if sq is None else sq[j * D:(j + 1) * D])
+            fold(L["wo"], p + "self_attn.o_proj", so)
             gu = L["wgu"].view(Fh, 2, D)                                   # rows [up_0, gate_0, up_1, gate_1, ...]
-            fold(gu[:, 0], p + "mlp.up_proj")
-            fold(gu[:, 1], p + "mlp.gate_proj")
-            fold(L["wdown"], p + "mlp.down_proj")
+            sgu = None if sgu is None else sgu.view(Fh, 2)
+            fold(gu[:, 0], p + "mlp.up_proj", None if sgu is None else sgu[:, 0])
+            fold(gu[:, 1], p + "mlp.gate_proj", None if sgu is None else sgu[:, 1])
+            fold(L["wdown"], p + "mlp.down_proj", sdown)
             setf(L["ln1"], p + "input_layernorm.weight")
             setf(L["ln2"], p + "post_attention_layernorm.weight")
         setf(self.norm, "model.norm.weight")
@@ -315,6 +354,24 @@ class LlamaForCausalLM:
         return self.kcache[li][pages].reshape(-1, D)[:n], self.vcache[li][pages].reshape(-1, D)[:n]
 
     # ---- prefill: tensor-core path ---------------------------------------------------------------------------------------
+    def _gemm(self, a, L, name, **kw):
+        """prefill projection a @ L[name]^T.  FP8 weights are first dequantized into the shared fp16 scratch buffer; the GEMM then reads a
+        B operand the previous kernel wrote, so it must not prefetch it before the PDL wait (dynamic_b)."""
+        s = L.get(name + "_s")
+        if s is None:
+            return ops.gemm(a, L[name], **kw)
+        w8 = L[name]
+        w = self._wscratch[:w8.numel()].view(w8.shape)
+        ops.dequant_fp8(w8, s, w)
+        return ops.gemm(a, w, dynamic_b=True, **kw)
+
+    def _gemv(self, L, name, x, out, **kw):
+        """token-loop projection: seedx_gemv_f16, or seedx_gemv_fp8 with the row scales of an FP8 matrix"""
+        s = L.get(name + "_s")
+        if s is not None:
+            kw["scale"] = s
+        return ops.gemv(L[name], x, out, **kw)
+
     def prefill(self, x, pos0=0, slot=0):
         """x: fp32 device [P, D] input embeddings for positions pos0.. of sequence slot `slot`; fills its KV cache; returns the fp32
         residual stream [P, D]."""
@@ -333,7 +390,7 @@ class LlamaForCausalLM:
         ov = o.view(1, P, H, d).permute(0, 2, 1, 3)
         for li, L in enumerate(self.layers):
             ops.layernorm(x, L["ln1"], None, cfg["eps"], out=n, rms=True)
-            ops.gemm(n, L["wqkv"], out=qkv)
+            self._gemm(n, L, "wqkv", out=qkv)
             ops.rope_kv_prefill(qkv, pos0, H, d, self.inv_freq, self.kcache[li], self.vcache[li], page_table_row=self.page_table[slot],
                                 page_size=self.page_size)
             if pos0 == 0:
@@ -342,10 +399,10 @@ class LlamaForCausalLM:
                 kc, vc = self.kv_rows(li, slot, pos0 + P)
                 ops.attention(qv, kc.view(1, pos0 + P, H, d).permute(0, 2, 1, 3), vc.view(1, pos0 + P, H, d).permute(0, 2, 1, 3), ov,
                               scale=d ** -0.5, causal=True)
-            ops.gemm(o, L["wo"], out=x, residual=x)
+            self._gemm(o, L, "wo", out=x, residual=x)
             ops.layernorm(x, L["ln2"], None, cfg["eps"], out=n, rms=True)
-            ops.gemm(n, L["wgu"], out=gu, act=ops.ACT_SILU, gated=True)
-            ops.gemm(gu, L["wdown"], out=x, residual=x)
+            self._gemm(n, L, "wgu", out=gu, act=ops.ACT_SILU, gated=True)
+            self._gemm(gu, L, "wdown", out=x, residual=x)
         return x
 
     def prefill_batch(self, xs, slots):
@@ -370,7 +427,7 @@ class LlamaForCausalLM:
         gu = torch.empty((T, cfg["ffn"]), device=x.device, dtype=torch.float16)
         for li, L in enumerate(self.layers):
             ops.layernorm(x, L["ln1"], None, cfg["eps"], out=n, rms=True)
-            ops.gemm(n, L["wqkv"], out=qkv)
+            self._gemm(n, L, "wqkv", out=qkv)
             for r, slot in enumerate(slots):
                 a, P = offs[r], lens[r]
                 blk = qkv[a:a + P]
@@ -379,10 +436,10 @@ class LlamaForCausalLM:
                 q4 = blk.view(1, P, 3, H, d)
                 qv, kv, vv = (q4[:, :, i].permute(0, 2, 1, 3) for i in range(3))
                 ops.attention(qv, kv, vv, o[a:a + P].view(1, P, H, d).permute(0, 2, 1, 3), scale=d ** -0.5, causal=True)
-            ops.gemm(o, L["wo"], out=x, residual=x)
+            self._gemm(o, L, "wo", out=x, residual=x)
             ops.layernorm(x, L["ln2"], None, cfg["eps"], out=n, rms=True)
-            ops.gemm(n, L["wgu"], out=gu, act=ops.ACT_SILU, gated=True)
-            ops.gemm(gu, L["wdown"], out=x, residual=x)
+            self._gemm(n, L, "wgu", out=gu, act=ops.ACT_SILU, gated=True)
+            self._gemm(gu, L, "wdown", out=x, residual=x)
         return [x[offs[r]:offs[r + 1]] for r in range(len(xs))]
 
     def logits_all(self, x):
@@ -393,18 +450,18 @@ class LlamaForCausalLM:
 
     # ---- token loop: HBM-bound path ----------------------------------------------------------------------------------------
     def _decode_step(self, hidden, img_ids, eos_id, suppress_eos):
-        """one token for every sequence slot: the fp16 weights are streamed once and shared by all slots"""
+        """one token for every sequence slot: the weights (fp16, or FP8 + row scales) are streamed once and shared by all slots"""
         cfg = self.cfg
         H = cfg["heads"]
         d = cfg["hidden"] // H
         ops.embed_rows(self.embed, self.xa, state=self.state, seq=self.seq)
         for li, L in enumerate(self.layers):
-            ops.gemv(L["wqkv"], self.xa, self.qkv1, rms_w=L["ln1"], eps=cfg["eps"])
+            self._gemv(L, "wqkv", self.xa, self.qkv1, rms_w=L["ln1"], eps=cfg["eps"])
             ops.decode_attention(self.qkv1, self.state, self.inv_freq, self.kcache[li], self.vcache[li], self.att1, H, d,
                                  page_table=self.page_table, page_size=self.page_size)
-            ops.gemv(L["wo"], self.att1, self.xb, residual=self.xa)
-            ops.gemv(L["wgu"], self.xb, self.g1, rms_w=L["ln2"], eps=cfg["eps"], gated=True)
-            ops.gemv(L["wdown"], self.g1, self.xa, residual=self.xb)
+            self._gemv(L, "wo", self.att1, self.xb, residual=self.xa)
+            self._gemv(L, "wgu", self.xb, self.g1, rms_w=L["ln2"], eps=cfg["eps"], gated=True)
+            self._gemv(L, "wdown", self.g1, self.xa, residual=self.xb)
         ops.layernorm(self.xa, self.norm, None, cfg["eps"], out=self.hn1, rms=True)
         ops.store_hidden(self.hn1, self.state, hidden)
         ops.gemv(self.lm_head, self.hn1, self.logits)

@@ -406,17 +406,36 @@ def cfg_euler_step(eps, x, unet_in, branches, guidance, image_guidance, sigma, s
     return x
 
 
-def gemv(W, x, out, *, rms_w=None, eps=1e-5, residual=None, gated=False):
-    """out[b] fp32 = epi(W[N,K] . (rmsnorm(x[b])*rms_w | x[b])); W fp16; x fp32 [K] or [B,K] with B in {1,2,4,8} (weights streamed once)."""
-    _require_cuda(W, x, out)
-    assert W.dtype == torch.float16 and W.is_contiguous() and x.dtype == torch.float32 and out.dtype == torch.float32
+def gemv(W, x, out, *, rms_w=None, eps=1e-5, residual=None, gated=False, scale=None):
+    """out[b] fp32 = epi(W[N,K] . (rmsnorm(x[b])*rms_w | x[b])); x fp32 [K] or [B,K] with B in {1,2,4,8} (weights streamed once).
+    W fp16, or float8_e4m3fn with scale = fp32 [N] (weight row n = scale[n] * W[n]; seedx_gemv_fp8)."""
+    _require_cuda(W, x, out, scale)
+    fp8 = W.dtype == torch.float8_e4m3fn
+    assert (W.dtype == torch.float16 and scale is None) or (fp8 and scale is not None)
+    assert W.is_contiguous() and x.dtype == torch.float32 and out.dtype == torch.float32
     N, K = W.shape
     x2 = x.reshape(-1, K)
     o2 = out.reshape(x2.shape[0], -1)
     r2 = residual.reshape(x2.shape[0], -1) if residual is not None else None
     assert x2.stride(1) == 1 and o2.stride(1) == 1
-    check(lib().seedx_gemv_f16(_ptr(W), _ptr(x2), _i64(x2.stride(0)), _ptr(rms_w), C.c_float(eps), _ptr(r2), _i64(r2.stride(0) if r2 is not None else 0),
-                               _ptr(o2), _i64(o2.stride(0)), _i64(N), _i64(K), C.c_int(x2.shape[0]), C.c_int(int(gated)), _stream()), "seedx_gemv_f16")
+    tail = (_ptr(x2), _i64(x2.stride(0)), _ptr(rms_w), C.c_float(eps), _ptr(r2), _i64(r2.stride(0) if r2 is not None else 0),
+            _ptr(o2), _i64(o2.stride(0)), _i64(N), _i64(K), C.c_int(x2.shape[0]), C.c_int(int(gated)), _stream())
+    if fp8:
+        assert scale.dtype == torch.float32 and scale.is_contiguous() and scale.numel() == N
+        check(lib().seedx_gemv_fp8(_ptr(W), _ptr(scale), *tail), "seedx_gemv_fp8")
+    else:
+        check(lib().seedx_gemv_f16(_ptr(W), *tail), "seedx_gemv_f16")
+    return out
+
+
+def dequant_fp8(W8, scale, out):
+    """fp16 out[n, k] = (half)(float(W8[n, k]) * scale[n]); W8 float8_e4m3fn [N, K], scale fp32 [N], out fp16 with W8's shape (all contiguous).
+    A GEMM that reads `out` right after this call must pass dynamic_b=True."""
+    _require_cuda(W8, scale, out)
+    assert W8.dtype == torch.float8_e4m3fn and W8.is_contiguous() and W8.dim() == 2
+    assert scale.dtype == torch.float32 and scale.is_contiguous() and scale.numel() == W8.shape[0]
+    assert out.dtype == torch.float16 and out.is_contiguous() and out.shape == W8.shape
+    check(lib().seedx_dequant_fp8(_ptr(W8), _ptr(scale), _ptr(out), _i64(W8.shape[0]), _i64(W8.shape[1]), _stream()), "seedx_dequant_fp8")
     return out
 
 
