@@ -126,6 +126,20 @@ void seedx_gemm_set_tma_epilogue(int on);
 /* what the most recent seedx_gemm_f16 launch ran, as decided on the host: out = {tile width, CTAs per cluster (1/2), stream-K (0/1),
  * TMA epilogue (0/1), 16-byte vector stores allowed for the direct epilogue (0/1), pipeline stages}; all zero before the first launch */
 void seedx_gemm_last_config(int32_t out[6]);
+/* The same GEMM on FP8 operands: A and B are e4m3 (OCP "fn" variant, float8_e4m3fn) with one fp32 scale per row of each, so that row m of the
+ * true A is a_scale[m] * A[m, :] and row n of the true B is b_scale[n] * B[n, :].  lda / ldb are in elements (= bytes); rows start 16-byte
+ * aligned (K % 16 == 0, lda % 16 == 0, ldb % 16 == 0).  The wgmma MMAs take 32 e4m3 values of K per step (QGMMA) at twice the fp16 rate.
+ * epilogue order: x = (acc * a_scale[m]) * b_scale[n]   (fp32, each product rounded), then exactly the seedx_gemm_f16 epilogue on x in place of
+ *                 the accumulator: x = alpha*x (or the folded-LayerNorm form rstd*x + bias - rstd*mean*colsum); biases; activation or gating;
+ *                 residual; store; row / column statistics.
+ * Every other field of args means what it means for seedx_gemm_f16.  Rejected (error, nothing launched): conv mode, batch != 1, a NULL scale,
+ * tile_n other than 0 (auto) / 64 / 128 / 160 / 192 / 224 / 256.  Runs single-CTA tiles with the data-parallel schedule only (no cluster pairs,
+ * no stream-K); seedx_gemm_last_config reports it like any other launch. */
+int seedx_gemm_fp8(const seedx_gemm_args* args, const float* a_scale, const float* b_scale, void* stream);
+/* Per-row FP8 quantisation of fp16 activations [rows, cols] (row stride ldx): scale[r] = amax_c |x[r, c]| / 448 (1 for an all-zero row) and
+ * q[r, c] = e4m3_rn(clamp(x[r, c] / scale[r], -448, 448)) with IEEE division, written to q (e4m3, row stride ldq bytes).  One read of the row,
+ * 16-byte loads and stores.  Requires ldx % 8 == 0, ldq % 16 == 0, 16-byte aligned x and q, cols <= 8192.  Feeds the A operand of seedx_gemm_fp8. */
+int seedx_quant_rows_fp8(const void* x, int64_t ldx, int64_t rows, int64_t cols, void* q, int64_t ldq, float* scale, void* stream);
 
 
 /* ------------------------------------------------------------------------------------------------

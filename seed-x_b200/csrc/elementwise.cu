@@ -63,6 +63,69 @@ __global__ void avgpool_tokens_kernel(const T* __restrict__ x, long long n_out_r
 }
 
 
+// Per-row FP8 (e4m3) quantisation of fp16 activations, the A operand of seedx_gemm_fp8: s = amax / 448 (1 for an all-zero row),
+// q = e4m3_rn(clamp(x / s, +-448)) with IEEE division.  One warp per row; a lane holds NV units of 16 columns (two 16-byte loads, one 16-byte
+// store) in registers between the row maximum and the conversion, so the row is read once.  Columns past the last whole unit (< 16) take one
+// lane each.
+SEEDX_DEVINL uint16_t f32x2_to_e4m3x2(float lo, float hi) {   // lo -> low byte (the lower column)
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;\n" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+SEEDX_DEVINL float fp8_quant_val(float x, float s) { return fminf(fmaxf(__fdiv_rn(x, s), -448.f), 448.f); }
+
+template <int NV>
+__global__ void __launch_bounds__(128)
+quant_rows_fp8_kernel(const __half* __restrict__ x, long long ldx, long long rows, int cols, uint8_t* __restrict__ q, long long ldq,
+                      float* __restrict__ scale) {
+  pdl_wait();
+  pdl_trigger();
+  const int lane = threadIdx.x & 31;
+  const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= rows) return;
+  const __half* xr = x + row * ldx;
+  uint8_t* qr = q + row * ldq;
+  const int units = cols >> 4;
+  uint4 v[NV][2];
+  __half2 mx = __float2half2_rn(0.f);
+#pragma unroll
+  for (int j = 0; j < NV; ++j) {
+    const int u = lane + 32 * j;
+    if (u < units) {
+      v[j][0] = __ldg((const uint4*)(xr + 16 * u));
+      v[j][1] = __ldg((const uint4*)(xr + 16 * u + 8));
+      const __half2* h0 = (const __half2*)&v[j][0];
+      const __half2* h1 = (const __half2*)&v[j][1];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) mx = __hmax2(mx, __hmax2(__habs2(h0[e]), __habs2(h1[e])));
+    }
+  }
+  const int tcol = 16 * units + lane;
+  const float tv = tcol < cols ? __half2float(xr[tcol]) : 0.f;
+  const float amax = warp_max(fmaxf(fmaxf(__low2float(mx), __high2float(mx)), fabsf(tv)));
+  float s = __fdiv_rn(amax, 448.f);
+  s = s > 0.f ? s : 1.f;
+  if (lane == 0) scale[row] = s;
+#pragma unroll
+  for (int j = 0; j < NV; ++j) {
+    const int u = lane + 32 * j;
+    if (u < units) {
+      uint32_t o[4];
+#pragma unroll
+      for (int w = 0; w < 4; ++w) {   // 4 output words of 4 values: halves 2w, 2w+1 of the 16
+        const uint4& src = v[j][w >> 1];
+        const uint32_t a0 = (w & 1) ? src.z : src.x, a1 = (w & 1) ? src.w : src.y;
+        const float2 f0 = __half22float2(*(const __half2*)&a0), f1 = __half22float2(*(const __half2*)&a1);
+        const uint32_t lo = f32x2_to_e4m3x2(fp8_quant_val(f0.x, s), fp8_quant_val(f0.y, s));
+        const uint32_t hi = f32x2_to_e4m3x2(fp8_quant_val(f1.x, s), fp8_quant_val(f1.y, s));
+        o[w] = lo | (hi << 16);
+      }
+      *(uint4*)(qr + 16 * u) = make_uint4(o[0], o[1], o[2], o[3]);
+    }
+  }
+  if (tcol < cols) qr[tcol] = (uint8_t)f32x2_to_e4m3x2(fp8_quant_val(tv, s), 0.f);
+}
+
 // im2col for strided convs on NHWC fp16 (k x k taps, stride s, pad_before on top/left, zero fill), 8 channels / thread
 __global__ void im2col_nhwc_kernel(const __half* __restrict__ x, int n, int h, int w, int c, int k, int stride, int pad, int ho, int wo,
                                    __half* __restrict__ out) {
@@ -295,6 +358,25 @@ extern "C" int seedx_cast(const void* src, int sd, void* dst, int dd, int64_t co
   else SEEDX_REQUIRE(false, "seedx_cast: unsupported conversion %d -> %d", sd, dd);
   count_launch();
   return check_cuda(cudaGetLastError(), "cast launch");
+}
+
+extern "C" int seedx_quant_rows_fp8(const void* x, int64_t ldx, int64_t rows, int64_t cols, void* q, int64_t ldq, float* scale, void* stream) {
+  SEEDX_REQUIRE(x && q && scale, "seedx_quant_rows_fp8: null pointer");
+  SEEDX_REQUIRE(rows > 0 && cols > 0 && cols <= 8192, "seedx_quant_rows_fp8: rows=%lld cols=%lld (1 <= cols <= 8192)", (long long)rows, (long long)cols);
+  SEEDX_REQUIRE(ldx >= cols && ldq >= cols && ldx % 8 == 0 && ldq % 16 == 0 && (uintptr_t)x % 16 == 0 && (uintptr_t)q % 16 == 0,
+                "seedx_quant_rows_fp8: rows must start 16-byte aligned (ldx %% 8 == 0, ldq %% 16 == 0, aligned pointers) and ldx, ldq >= cols");
+  const int per_lane = (int)((cols / 16 + 31) / 32);
+  const dim3 grid((unsigned)((rows + 3) / 4));
+  cudaStream_t st = (cudaStream_t)stream;
+  const __half* xp = (const __half*)x;
+  uint8_t* qp = (uint8_t*)q;
+  if (per_lane <= 1) launch_k(quant_rows_fp8_kernel<1>, grid, 128, 0, st, xp, (long long)ldx, (long long)rows, (int)cols, qp, (long long)ldq, scale);
+  else if (per_lane <= 2) launch_k(quant_rows_fp8_kernel<2>, grid, 128, 0, st, xp, (long long)ldx, (long long)rows, (int)cols, qp, (long long)ldq, scale);
+  else if (per_lane <= 4) launch_k(quant_rows_fp8_kernel<4>, grid, 128, 0, st, xp, (long long)ldx, (long long)rows, (int)cols, qp, (long long)ldq, scale);
+  else if (per_lane <= 8) launch_k(quant_rows_fp8_kernel<8>, grid, 128, 0, st, xp, (long long)ldx, (long long)rows, (int)cols, qp, (long long)ldq, scale);
+  else launch_k(quant_rows_fp8_kernel<16>, grid, 128, 0, st, xp, (long long)ldx, (long long)rows, (int)cols, qp, (long long)ldq, scale);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "quant_rows_fp8 launch");
 }
 
 extern "C" int seedx_avgpool_tokens(const void* x, int dtype, int64_t n, int64_t t, int64_t c, int64_t k, void* out, void* stream) {

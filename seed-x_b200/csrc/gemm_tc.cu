@@ -1,6 +1,7 @@
 // seedx-b200: wgmma tensor-core GEMM / implicit-GEMM convolution for sm_90a.
 //
 //   D[b][m][n] = epi( alpha * sum_k A[b][m][k] * B[b][n][k] )      fp16 operands, fp32 accumulate in registers
+//   D[m][n]    = epi( alpha * acc[m][n] * a_scale[m] * b_scale[n] )  FP8 variant (seedx_gemm_fp8): e4m3 operands, per-row scales
 //
 // Persistent, warp-specialised: warpgroup 0 = TMA producer, warpgroups 1 and 2 = wgmma on 64 rows each of the 128-row tile, then the epilogue.
 // Operands are staged by TMA into 128B-swizzled K-major tiles (BM=128 x BK=64, BN x BK=64) through a
@@ -10,8 +11,10 @@
 // (im2col-free implicit GEMM).
 //
 // Reference call sites replaced: see include/seedx.h (seedx_gemm_f16).
+#include <cuda_fp8.h>
 #include <math.h>
 #include <cstdlib>
+#include <type_traits>
 
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -58,6 +61,9 @@ struct GemmParams {
   float row_eps;
   // conv
   int conv, taps_w, c_chunks, conv_w, conv_h, tile_w, tile_h, tiles_per_img, tiles_w, pad, imgs_per_tile;
+  // FP8 (e4m3) operands only: the accumulator is scaled by a_scale[m] * b_scale[n] before the rest of the epilogue
+  const float* a_scale;                   // [M]
+  const float* b_scale;                   // [N]
 };
 
 constexpr int BM = 128;
@@ -70,7 +76,8 @@ constexpr int SMEM_LIMIT = 227 * 1024;
 constexpr int EPI_OUT_BYTES = 4096;                      // per epilogue warp: output tiles (2 x <=2 KB, or 1 x 4 KB)
 constexpr int EPI_RES_BYTES = 8192;                      // per epilogue warp: residual tiles, ideally every chunk of a 256-wide tile in flight
 constexpr int MAX_STAGES = 8;
-constexpr int VEC_BYTES = 1024;                          // one per-tile column vector of the epilogue (bias_n | LayerNorm column sums), 256 fp32
+constexpr int VEC_BYTES = 1024;                          // one per-tile column vector of the epilogue (bias_n | LayerNorm column sums | FP8 b_scale), 256 fp32
+constexpr int BK_FP8 = 128;                              // e4m3 K elements per stage: 128 bytes per row, the same tile bytes and swizzle as 64 fp16
 // The epilogue works on rows of 32 accumulator columns (lane = row).  The accumulators live in the wgmma fragment layout (a thread holds 2 rows x
 // 2 columns of every 8-column group), so each warpgroup passes 64 columns at a time through shared memory: 64 rows x ACC_LD fp32.
 // ACC_LD = 72: the fragment's 8-byte stores hit 32 distinct banks per half warp.
@@ -142,11 +149,15 @@ SEEDX_DEVINL bool seg_next(const GemmParams& p, SegState& s, int n_clusters, int
 // 128 rows of A and HALF of the B tile, which TMA multicasts into both CTAs' shared memory: each SM fetches a quarter fewer operand bytes from L2.
 // A stage of a CTA is refilled only when the consumers of BOTH CTAs have released it (the peer writes into it), so every consumer warpgroup
 // arrives on the `empty` barriers of both CTAs.
-template <int BN, int CL, bool SK>
+// TE = operand element type: __half, or __nv_fp8_e4m3 (single CTA, data-parallel, plain GEMM only: the host never instantiates FP8 with CL = 2,
+// stream-K or conv mode).  Every FP8 difference is under `if constexpr`, so the fp16 kernels are the same code with or without it.
+template <int BN, int CL, bool SK, typename TE = __half>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmD,
                const __grid_constant__ CUtensorMap tmR, const GemmParams p) {
   using Cfg = TileCfg<BN, CL>;
+  constexpr bool FP8 = std::is_same<TE, __nv_fp8_e4m3>::value;
+  constexpr int KB = FP8 ? BK_FP8 : BK;   // K elements per stage (TMA box coordinate step)
   const int STAGES = p.stages;
   if (threadIdx.x == 0) GEMM_STAMP(0);
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -159,7 +170,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
   auto res_bar = [&](int w, int i) { return bar_base + 8u * (2 * STAGES + 4 * w + i); };  // residual tile landed (per epilogue warp, <= 4 buffers)
-  const uint32_t vec_base = bar_base + 512u;       // [bias_n tile | colsum tile], 256 fp32 each: staged once per tile, read as broadcast 128-bit loads
+  const uint32_t vec_base = bar_base + 512u;       // [bias_n tile | colsum tile | FP8: b_scale tile], 256 fp32 each: staged once per tile, read as broadcast 128-bit loads
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -186,8 +197,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int tile0 = (int)blockIdx.x / CL, tile_step = (int)gridDim.x / CL;
   // B half of a stage: rows [n_blk*BN + crank*BN/CL, +BN/CL), at the same offset in every CTA of the cluster
   auto load_b = [&](uint32_t sb, uint32_t bar, int kb, int n_blk, int b) {
-    if (CL == 1) tma_load_3d(sb, &tmB, bar, kb * BK, n_blk * BN, p.b_batched ? b : 0);
-    else tma_load_3d_mc(sb + (uint32_t)(crank * (BN / CL) * BK * 2), &tmB, bar, kb * BK, n_blk * BN + crank * (BN / CL), p.b_batched ? b : 0,
+    if (CL == 1) tma_load_3d(sb, &tmB, bar, kb * KB, n_blk * BN, p.b_batched ? b : 0);
+    else tma_load_3d_mc(sb + (uint32_t)(crank * (BN / CL) * BK * 2), &tmB, bar, kb * KB, n_blk * BN + crank * (BN / CL), p.b_batched ? b : 0,
                         (uint16_t)((1u << CL) - 1u));
   };
   // Weights never depend on the kernel before this one: the B tiles of the first stages of this CTA's first tile are requested BEFORE the
@@ -253,7 +264,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             const int kw = tap - kh * p.taps_w;
             tma_load_4d(sa, &tmA, full_bar(stage), cc * BK, w0 + kw - p.pad, h0 + kh - p.pad, img);
           } else {
-            tma_load_3d(sa, &tmA, full_bar(stage), kb * BK, m_blk * BM, b);
+            tma_load_3d(sa, &tmA, full_bar(stage), kb * KB, m_blk * BM, b);
           }
           if (!b_done) load_b(sb, full_bar(stage), kb, n_blk, b);
           if (++stage == STAGES) {
@@ -312,8 +323,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           wgmma_fence_regs<BN / 2>(acc);
           wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k)   // advance 16 fp16 = 32 B inside the 128B swizzle atom: +2 in the (addr >> 4) field
-            wgmma_ss_n<BN>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), ((kb - kb0) | k) != 0);
+          for (int k = 0; k < BK / 16; ++k) {  // advance 16 fp16 (or 32 e4m3) = 32 B inside the 128B swizzle atom: +2 in the (addr >> 4) field
+            if constexpr (FP8) wgmma_ss_e4m3<BN>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), ((kb - kb0) | k) != 0);
+            else wgmma_ss_n<BN>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), ((kb - kb0) | k) != 0);
+          }
           wgmma_commit();
           wgmma_wait<1>();
           wgmma_fence_regs<BN / 2>(acc);
@@ -364,6 +377,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       };
 
       const float bm = (p.bias_m != nullptr && row_ok) ? p.bias_m[row] : 0.f;
+      float a_s = 1.f;                         // FP8: the scale of this lane's row of A
+      if constexpr (FP8) a_s = row_ok ? __ldg(p.a_scale + row) : 0.f;
       float ln_rstd = 1.f, ln_nmr = 0.f;       // folded LayerNorm: x = rstd * acc + (-mean * rstd) * colsum[n]
       if (p.ln_stats != nullptr && row_ok) {
         float2 mr;
@@ -438,7 +453,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       // column vectors of this tile -> shared memory: the chunk loop then reads them with broadcast 128-bit shared loads instead of dependent
       // L1/L2 round trips per chunk
       const int vec_key = n_blk + (bg_vec ? (bg_grp + 1) * 65536 : 0);
-      const bool use_vec = (p.bias_n != nullptr || p.ln_stats != nullptr || bg_vec) && vec_key != vec_nblk;   // consecutive tiles of a CTA mostly differ in m only
+      const bool use_vec = (p.bias_n != nullptr || p.ln_stats != nullptr || bg_vec || FP8) && vec_key != vec_nblk;   // consecutive tiles of a CTA mostly differ in m only
       if (use_vec) {
         vec_nblk = vec_key;
         named_bar_sync(1, EPI_WARPS * 32);      // every epilogue warp has finished reading the previous tile's vectors
@@ -449,6 +464,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           const float cv = (p.ln_stats != nullptr && in) ? __ldg(p.ln_colsum + n0 + i) : 0.f;
           asm volatile("st.shared.f32 [%0], %1;\n" ::"r"(vec_base + 4u * (uint32_t)i), "f"(bv) : "memory");
           if (p.ln_stats != nullptr) asm volatile("st.shared.f32 [%0], %1;\n" ::"r"(vec_base + 1024u + 4u * (uint32_t)i), "f"(cv) : "memory");
+          if constexpr (FP8) {
+            const float sv = in ? __ldg(p.b_scale + n0 + i) : 0.f;
+            asm volatile("st.shared.f32 [%0], %1;\n" ::"r"(vec_base + 2048u + 4u * (uint32_t)i), "f"(sv) : "memory");
+          }
         }
         named_bar_sync(1, EPI_WARPS * 32);
       }
@@ -476,6 +495,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               v[i] = __float_as_uint(__uint_as_float(v[i]) + qv.x), v[i + 1] = __float_as_uint(__uint_as_float(v[i + 1]) + qv.y);
               v[i + 2] = __float_as_uint(__uint_as_float(v[i + 2]) + qv.z), v[i + 3] = __float_as_uint(__uint_as_float(v[i + 3]) + qv.w);
             }
+          }
+        }
+        if constexpr (FP8) {       // acc <- (acc * a_scale[m]) * b_scale[n], then the fp16 epilogue below, unchanged
+#pragma unroll
+          for (int i = 0; i < 32; i += 4) {
+            const uint4 qs = lds128(vec_base + 2048u + 4u * (uint32_t)(c + i));
+            v[i] = __float_as_uint(__uint_as_float(v[i]) * a_s * __uint_as_float(qs.x));
+            v[i + 1] = __float_as_uint(__uint_as_float(v[i + 1]) * a_s * __uint_as_float(qs.y));
+            v[i + 2] = __float_as_uint(__uint_as_float(v[i + 2]) * a_s * __uint_as_float(qs.z));
+            v[i + 3] = __float_as_uint(__uint_as_float(v[i + 3]) * a_s * __uint_as_float(qs.w));
           }
         }
         float x[32];
@@ -747,21 +776,24 @@ constexpr size_t SK_FLAG_BYTES = 16384;
 // what the most recent launch ran (seedx_gemm_last_config): tile width, cluster size, stream-K, TMA epilogue, vec_ok, pipeline stages
 static int g_gemm_last[6] = {0, 0, 0, 0, 0, 0};
 
-template <int BN, int CL>
+template <int BN, int CL, typename TE = __half>
 static int launch_gemm_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& td, const CUtensorMap& tr, const GemmParams& p_in,
                           cudaStream_t st) {
   using Cfg = TileCfg<BN, CL>;
+  constexpr bool kFP8 = std::is_same<TE, __nv_fp8_e4m3>::value;
   // stream-K kernels exist for cluster pairs with 32-column-multiple tiles of at least 128 columns (where the schedule is ever chosen)
-  constexpr bool kHasSK = (CL == 2) && (BN % 32 == 0) && (BN >= 128);
+  constexpr bool kHasSK = (CL == 2) && (BN % 32 == 0) && (BN >= 128) && !kFP8;
   static bool attr_done = false;
   if (!attr_done) {
-    SEEDX_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, CL, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
-    if (kHasSK) SEEDX_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, CL, kHasSK>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
+    SEEDX_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, CL, false, TE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
+    if (kHasSK) SEEDX_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, CL, kHasSK, TE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
     attr_done = true;
   }
   GemmParams p = p_in;
   int epi_bytes = EPI_WARPS * p.epi_warp_bytes;
-  const int tail_bytes = 512 + (p.bias_n != nullptr || p.ln_stats != nullptr || p.bias_g != nullptr ? VEC_BYTES : 0) + (p.ln_stats != nullptr ? VEC_BYTES : 0);
+  // FP8 stages the b_scale vector behind the bias and column-sum slots, so it budgets all three
+  const int tail_bytes = kFP8 ? 512 + 3 * VEC_BYTES
+                              : 512 + (p.bias_n != nullptr || p.ln_stats != nullptr || p.bias_g != nullptr ? VEC_BYTES : 0) + (p.ln_stats != nullptr ? VEC_BYTES : 0);
   p.stages = Cfg::stages_for(epi_bytes, tail_bytes);
   if (p.stages < 3 && p.tma_epi && p.epi_warp_bytes > 32 * p.epi_row_bytes * (p.epi_res_bytes ? 2 : 1)) {
     // the short-K staging (several boxes in flight per warp) would leave a wide tile fewer than three pipeline stages: one box each
@@ -772,7 +804,7 @@ static int launch_gemm_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CU
     p.stages = Cfg::stages_for(epi_bytes, tail_bytes);
   }
   if (p.stages < 2) {
-    set_error("seedx_gemm_f16: tile %dx%d does not fit in shared memory with %d B of epilogue staging", BM * CL, BN, epi_bytes);
+    set_error("%s: tile %dx%d does not fit in shared memory with %d B of epilogue staging", kFP8 ? "seedx_gemm_fp8" : "seedx_gemm_f16", BM * CL, BN, epi_bytes);
     return 5;
   }
   const int smem_bytes = Cfg::smem_for(p.stages, epi_bytes, tail_bytes);
@@ -788,7 +820,7 @@ static int launch_gemm_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CU
       qa[0].id = cudaLaunchAttributeClusterDimension;
       qa[0].val.clusterDim.x = CL, qa[0].val.clusterDim.y = 1, qa[0].val.clusterDim.z = 1;
       q.attrs = qa, q.numAttrs = 1;
-      SEEDX_CUDA(cudaOccupancyMaxActiveClusters(&occ_clusters, gemm_tc_kernel<BN, CL, false>, &q));
+      SEEDX_CUDA(cudaOccupancyMaxActiveClusters(&occ_clusters, gemm_tc_kernel<BN, CL, false, TE>, &q));
       occ_smem = smem_bytes;
     }
     if (occ_clusters > 0 && occ_clusters < max_clusters) max_clusters = occ_clusters;
@@ -825,8 +857,8 @@ static int launch_gemm_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CU
   cfg.attrs = attr;
   cfg.numAttrs = pdl_enabled() ? 2 : 1;
   g_gemm_last[0] = BN, g_gemm_last[1] = CL, g_gemm_last[2] = p.stream_k, g_gemm_last[3] = p.tma_epi, g_gemm_last[4] = p.vec_ok, g_gemm_last[5] = p.stages;
-  const cudaError_t e = (kHasSK && p.stream_k) ? cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, CL, kHasSK>, ta, tb, td, tr, p)
-                                               : cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, CL, false>, ta, tb, td, tr, p);
+  const cudaError_t e = (kHasSK && p.stream_k) ? cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, CL, kHasSK, TE>, ta, tb, td, tr, p)
+                                               : cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, CL, false, TE>, ta, tb, td, tr, p);
   count_launch();
   return check_cuda(e != cudaSuccess ? e : cudaGetLastError(), "gemm_tc_kernel launch");
 }
@@ -855,6 +887,8 @@ static bool valid_tile_n(int bn) {
 // MMA: a 128 x BN x 16 step is BN cycles at the dense fp16 rate of an H100 SM (2048 FMA/clk), divided by the rate a tile width reaches
 // relative to the 256-wide tile.  Measured on an H100 SXM at 700 W, 8192^3 single-CTA launches (256 wide: 616 TFLOP/s): narrower tiles
 // re-read A more often per FLOP and leave more stages' worth of latency exposed, widths that are not one wgmma instruction issue several.
+// The FP8 GEMM reuses this table with k_blocks counted in its 128-element stages (one stage = the MMA time of a 64-element fp16 stage at twice
+// the rate).  The rates were measured for fp16, not for FP8.
 struct TileRate {
   int bn;
   double rate;
@@ -911,19 +945,32 @@ extern "C" int seedx_gemm_set_workspace(void* ptr, int64_t bytes) {
   return 0;
 }
 
-extern "C" int seedx_gemm_f16(const seedx_gemm_args* a, void* stream) {
-  SEEDX_REQUIRE(a != nullptr, "seedx_gemm_f16: null args");
-  SEEDX_REQUIRE(a->A && a->B && a->D, "seedx_gemm_f16: null operand pointer");
-  SEEDX_REQUIRE(a->M > 0 && a->N > 0 && a->K > 0 && a->batch > 0, "seedx_gemm_f16: empty problem M=%lld N=%lld K=%lld",
+// seedx_gemm_f16 and seedx_gemm_fp8: one host path.  FP8 differs in the element size (1 byte), the K per stage (128), the tensor-map type and the
+// scales; it runs single-CTA, data-parallel, batch 1, plain GEMM only, at the widths the auto chooser returns (and 64).
+static int gemm_entry(const seedx_gemm_args* a, bool fp8, const float* a_scale, const float* b_scale, void* stream) {
+  const char* fn = fp8 ? "seedx_gemm_fp8" : "seedx_gemm_f16";
+  SEEDX_REQUIRE(a != nullptr, "%s: null args", fn);
+  SEEDX_REQUIRE(a->A && a->B && a->D, "%s: null operand pointer", fn);
+  SEEDX_REQUIRE(a->M > 0 && a->N > 0 && a->K > 0 && a->batch > 0, "%s: empty problem M=%lld N=%lld K=%lld", fn,
                 (long long)a->M, (long long)a->N, (long long)a->K);
-  SEEDX_REQUIRE(a->K % 8 == 0, "seedx_gemm_f16: K=%lld must be a multiple of 8 (16-byte TMA rows)", (long long)a->K);
-  SEEDX_REQUIRE(((uintptr_t)a->A % 16 == 0) && ((uintptr_t)a->B % 16 == 0), "seedx_gemm_f16: operands must be 16B aligned");
-  SEEDX_REQUIRE(a->out_dtype == SEEDX_F16 || a->out_dtype == SEEDX_F32, "seedx_gemm_f16: bad out_dtype");
+  const int es = fp8 ? 1 : 2;                 // operand element bytes
+  const int kb_elems = fp8 ? BK_FP8 : BK;     // K elements per pipeline stage
+  const int row_align = 16 / es;              // elements per 16 bytes: TMA rows start and end on 16-byte boundaries
+  if (fp8) {
+    SEEDX_REQUIRE(a->conv_taps_h == 0 && a->conv_taps_w == 0, "seedx_gemm_fp8: conv mode is not supported");
+    SEEDX_REQUIRE(a->batch == 1, "seedx_gemm_fp8: batch=%lld, only batch 1 is supported", (long long)a->batch);
+    SEEDX_REQUIRE(a_scale != nullptr && b_scale != nullptr, "seedx_gemm_fp8: a_scale and b_scale are required");
+    SEEDX_REQUIRE(a->tile_n == 0 || a->tile_n == 64 || a->tile_n == 128 || a->tile_n == 160 || a->tile_n == 192 || a->tile_n == 224 || a->tile_n == 256,
+                  "seedx_gemm_fp8: tile_n must be 0 (auto) or one of 64/128/160/192/224/256");
+  }
+  SEEDX_REQUIRE(a->K % row_align == 0, "%s: K=%lld must be a multiple of %d (16-byte TMA rows)", fn, (long long)a->K, row_align);
+  SEEDX_REQUIRE(((uintptr_t)a->A % 16 == 0) && ((uintptr_t)a->B % 16 == 0), "%s: operands must be 16B aligned", fn);
+  SEEDX_REQUIRE(a->out_dtype == SEEDX_F16 || a->out_dtype == SEEDX_F32, "%s: bad out_dtype", fn);
   const bool conv = a->conv_taps_h > 0;
   GemmParams p{};
   int bn = a->tile_n;
-  SEEDX_REQUIRE(bn == 0 || valid_tile_n(bn), "seedx_gemm_f16: tile_n must be 0 (auto) or one of 64/96/128/144/160/192/208/224/240/256");
-  if (a->gated) SEEDX_REQUIRE(a->N % 2 == 0, "seedx_gemm_f16: gated epilogue needs even N");
+  SEEDX_REQUIRE(bn == 0 || valid_tile_n(bn), "%s: tile_n must be 0 (auto) or one of 64/96/128/144/160/192/208/224/240/256", fn);
+  if (a->gated) SEEDX_REQUIRE(a->N % 2 == 0, "%s: gated epilogue needs even N", fn);
 
   // ---- TMA epilogue eligibility (output / residual tiles go through shared memory and cp.async.bulk.tensor stores)
   const int out_es = a->out_dtype == SEEDX_F32 ? 4 : 2;
@@ -940,15 +987,15 @@ extern "C" int seedx_gemm_f16(const seedx_gemm_args* a, void* stream) {
   CUtensorMap ta, tb, td, tr;
   int cl = 1;
   if (!conv) {
-    SEEDX_REQUIRE(a->lda % 8 == 0 && a->lda >= a->K, "seedx_gemm_f16: lda must be >= K and a multiple of 8");
+    SEEDX_REQUIRE(a->lda % row_align == 0 && a->lda >= a->K, "%s: lda must be >= K and a multiple of %d", fn, row_align);
     uint64_t dims[3] = {(uint64_t)a->K, (uint64_t)a->M, (uint64_t)a->batch};
-    uint64_t bstride = a->batch > 1 ? (uint64_t)a->strideA * 2 : (uint64_t)a->lda * 2 * (uint64_t)a->M;
-    SEEDX_REQUIRE(bstride % 16 == 0, "seedx_gemm_f16: strideA must be a multiple of 8 elements");
-    uint64_t strides[2] = {(uint64_t)a->lda * 2, bstride};
-    uint32_t box[3] = {BK, BM, 1};
-    if (int e = encode_tmap(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, a->A, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))
+    uint64_t bstride = a->batch > 1 ? (uint64_t)a->strideA * es : (uint64_t)a->lda * es * (uint64_t)a->M;
+    SEEDX_REQUIRE(bstride % 16 == 0, "%s: strideA must be a multiple of 8 elements", fn);
+    uint64_t strides[2] = {(uint64_t)a->lda * es, bstride};
+    uint32_t box[3] = {(uint32_t)kb_elems, BM, 1};
+    if (int e = encode_tmap(&ta, fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, a->A, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))
       return e;
-    p.k_blocks = (int)((a->K + BK - 1) / BK);
+    p.k_blocks = (int)((a->K + kb_elems - 1) / kb_elems);   // the K tail of the last stage is TMA zero fill
     p.m_blocks = (int)((a->M + BM - 1) / BM);
     if (bn == 0) bn = choose_tile_n(p.m_blocks * (int)a->batch, (int)a->N, p.k_blocks, a->act != SEEDX_ACT_NONE, tma_epi);
   } else {
@@ -993,49 +1040,50 @@ extern "C" int seedx_gemm_f16(const seedx_gemm_args* a, void* stream) {
     p.m_blocks = (int)((a->M + BM - 1) / BM);
   }
   {
-    SEEDX_REQUIRE(a->ldb % 8 == 0 && a->ldb >= a->K, "seedx_gemm_f16: ldb must be >= K and a multiple of 8");
+    SEEDX_REQUIRE(a->ldb % row_align == 0 && a->ldb >= a->K, "%s: ldb must be >= K and a multiple of %d", fn, row_align);
     const bool bb = a->batch > 1 && a->strideB != 0;
     uint64_t dims[3] = {(uint64_t)a->K, (uint64_t)a->N, (uint64_t)(bb ? a->batch : 1)};
-    uint64_t bstride = bb ? (uint64_t)a->strideB * 2 : (uint64_t)a->ldb * 2 * (uint64_t)a->N;
-    SEEDX_REQUIRE(bstride % 16 == 0, "seedx_gemm_f16: strideB must be a multiple of 8 elements");
-    uint64_t strides[2] = {(uint64_t)a->ldb * 2, bstride};
+    uint64_t bstride = bb ? (uint64_t)a->strideB * es : (uint64_t)a->ldb * es * (uint64_t)a->N;
+    SEEDX_REQUIRE(bstride % 16 == 0, "%s: strideB must be a multiple of 8 elements", fn);
+    uint64_t strides[2] = {(uint64_t)a->ldb * es, bstride};
     // cluster pairs (B tile multicast in two halves, 16-row aligned) only when forced: on an H100 SXM (700 W) they measured about half the
     // single-CTA rate on every shape tried (8192 x {10240, 1280, 8192} x {1280, 5120, 8192}), so auto mode keeps single-CTA tiles
-    if (g_gemm_cluster == 2 && p.m_blocks >= 2 && bn % 32 == 0) cl = 2;
+    if (g_gemm_cluster == 2 && p.m_blocks >= 2 && bn % 32 == 0 && !fp8) cl = 2;
     // a single CTA with residual staging (96 KB) keeps only 2 stages of a 256-wide tile: use a narrower tile there
     if (cl == 1 && tma_epi && a->residual && bn > 160 && a->tile_n == 0) bn = 160;
-    uint32_t box[3] = {BK, (uint32_t)(bn / cl), 1};
-    if (int e = encode_tmap(&tb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, a->B, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))
+    uint32_t box[3] = {(uint32_t)kb_elems, (uint32_t)(bn / cl), 1};
+    if (int e = encode_tmap(&tb, fp8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, a->B, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))
       return e;
     p.b_batched = bb ? 1 : 0;
   }
   p.D = a->D;
   p.dbg = g_gemm_dbg;
+  p.a_scale = a_scale, p.b_scale = b_scale;
   if (a->ln_stats || a->ln_colsum) {
-    SEEDX_REQUIRE(a->ln_stats && a->ln_colsum, "seedx_gemm_f16: ln_stats and ln_colsum go together");
+    SEEDX_REQUIRE(a->ln_stats && a->ln_colsum, "%s: ln_stats and ln_colsum go together", fn);
     SEEDX_REQUIRE(a->batch == 1 && !conv && ((uintptr_t)a->ln_colsum % 16 == 0) && ((uintptr_t)a->ln_stats % 8 == 0) && a->N % 4 == 0,
-                  "seedx_gemm_f16: folded LayerNorm needs a plain un-batched GEMM, N %% 4 == 0 and aligned statistics");
-    SEEDX_REQUIRE(a->alpha == 1.0f && a->bias_m == nullptr, "seedx_gemm_f16: folded LayerNorm takes alpha = 1 and no per-row bias");
+                  "%s: folded LayerNorm needs a plain un-batched GEMM, N %% 4 == 0 and aligned statistics", fn);
+    SEEDX_REQUIRE(a->alpha == 1.0f && a->bias_m == nullptr, "%s: folded LayerNorm takes alpha = 1 and no per-row bias", fn);
   }
   p.ln_stats = (const float2*)a->ln_stats, p.ln_colsum = a->ln_colsum;
   p.ln_parts = a->ln_parts, p.ln_eps = a->ln_eps, p.ln_inv_cols = a->ln_parts > 0 ? 1.0f / (32.0f * (float)a->ln_parts) : 0.f;
   SEEDX_REQUIRE(a->ln_parts >= 0 && (a->ln_parts == 0 || (a->ln_stats && 32LL * a->ln_parts == a->K)),
-                "seedx_gemm_f16: ln_parts=%d must cover K=%lld columns in 32-column chunks", a->ln_parts, (long long)a->K);
+                "%s: ln_parts=%d must cover K=%lld columns in 32-column chunks", fn, a->ln_parts, (long long)a->K);
   if (a->row_part || a->col_part) {
     SEEDX_REQUIRE(tma_epi && !a->gated && a->out_dtype == SEEDX_F16 && a->batch == 1 && a->N % 32 == 0 && a->M % 32 == 0,
-                  "seedx_gemm_f16: output statistics need the TMA epilogue (16-byte aligned fp16 output), no gating, batch 1, M and N multiples of 32");
-    SEEDX_REQUIRE(((uintptr_t)a->row_part % 8 == 0) && ((uintptr_t)a->col_part % 8 == 0), "seedx_gemm_f16: statistics buffers must be 8-byte aligned");
+                  "%s: output statistics need the TMA epilogue (16-byte aligned fp16 output), no gating, batch 1, M and N multiples of 32", fn);
+    SEEDX_REQUIRE(((uintptr_t)a->row_part % 8 == 0) && ((uintptr_t)a->col_part % 8 == 0), "%s: statistics buffers must be 8-byte aligned", fn);
   }
   p.row_part = (float2*)a->row_part, p.col_part = (float2*)a->col_part;
   if (a->row_stats_out || a->row_tickets) {
     SEEDX_REQUIRE(a->row_part && a->row_stats_out && a->row_tickets && ((uintptr_t)a->row_stats_out % 8 == 0),
-                  "seedx_gemm_f16: row_stats_out needs row_part and row_tickets (M/32 zeroed counters)");
+                  "%s: row_stats_out needs row_part and row_tickets (M/32 zeroed counters)", fn);
   }
   p.row_stats_out = (float2*)a->row_stats_out, p.row_tickets = a->row_tickets, p.row_eps = a->row_eps;
   p.b_static = a->b_dynamic ? 0 : 1;
   p.bias_n = a->bias_n, p.bias_m = a->bias_m, p.bias_g = a->bias_g;
   p.bias_g_rows = a->bias_g ? (int)a->bias_g_rows : 1;
-  SEEDX_REQUIRE(p.bias_g_rows > 0, "seedx_gemm_f16: bias_g_rows must be > 0");
+  SEEDX_REQUIRE(p.bias_g_rows > 0, "%s: bias_g_rows must be > 0", fn);
   p.residual = a->residual;
   p.M = (int)a->M, p.N = (int)a->N, p.K = (int)a->K, p.batch = (int)a->batch;
   p.n_blocks = (int)((a->N + bn - 1) / bn);
@@ -1045,7 +1093,7 @@ extern "C" int seedx_gemm_f16(const seedx_gemm_args* a, void* stream) {
   p.act = a->act, p.gated = a->gated;
   p.out_f32 = a->out_dtype == SEEDX_F32;
   p.res_f32 = a->residual_dtype == SEEDX_F32;
-  if (a->residual) SEEDX_REQUIRE(a->residual_dtype == SEEDX_F16 || a->residual_dtype == SEEDX_F32, "seedx_gemm_f16: bad residual_dtype");
+  if (a->residual) SEEDX_REQUIRE(a->residual_dtype == SEEDX_F16 || a->residual_dtype == SEEDX_F32, "%s: bad residual_dtype", fn);
   // vector epilogue needs 16-byte aligned rows on D (and residual)
   const int oe = p.out_f32 ? 4 : 8;
   bool vec = ((uintptr_t)a->D % 16 == 0) && (a->ldd % oe == 0) && (a->strideD % oe == 0);
@@ -1089,6 +1137,16 @@ extern "C" int seedx_gemm_f16(const seedx_gemm_args* a, void* stream) {
     }
   }
   cudaStream_t st = (cudaStream_t)stream;
+  if (fp8) {
+    switch (bn) {
+      case 64: return launch_gemm_cl<64, 1, __nv_fp8_e4m3>(ta, tb, td, tr, p, st);
+      case 128: return launch_gemm_cl<128, 1, __nv_fp8_e4m3>(ta, tb, td, tr, p, st);
+      case 160: return launch_gemm_cl<160, 1, __nv_fp8_e4m3>(ta, tb, td, tr, p, st);
+      case 192: return launch_gemm_cl<192, 1, __nv_fp8_e4m3>(ta, tb, td, tr, p, st);
+      case 224: return launch_gemm_cl<224, 1, __nv_fp8_e4m3>(ta, tb, td, tr, p, st);
+      default: return launch_gemm_cl<256, 1, __nv_fp8_e4m3>(ta, tb, td, tr, p, st);
+    }
+  }
   switch (bn) {
     case 64: return launch_gemm<64>(ta, tb, td, tr, p, cl, st);
     case 96: return launch_gemm<96>(ta, tb, td, tr, p, cl, st);
@@ -1101,4 +1159,10 @@ extern "C" int seedx_gemm_f16(const seedx_gemm_args* a, void* stream) {
     case 240: return launch_gemm<240>(ta, tb, td, tr, p, cl, st);
     default: return launch_gemm<256>(ta, tb, td, tr, p, cl, st);
   }
+}
+
+extern "C" int seedx_gemm_f16(const seedx_gemm_args* a, void* stream) { return gemm_entry(a, false, nullptr, nullptr, stream); }
+
+extern "C" int seedx_gemm_fp8(const seedx_gemm_args* a, const float* a_scale, const float* b_scale, void* stream) {
+  return gemm_entry(a, true, a_scale, b_scale, stream);
 }

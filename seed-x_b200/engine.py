@@ -21,10 +21,11 @@ VIT_G = dict(width=1664, layers=48, heads=16, mlp_width=8192, output_dim=4096, n
 
 class SeedXEngine:
     def __init__(self, vit_cfg=None, llm_cfg=None, unet_cfg=None, vae_cfg=None, rxl_cfg=None, device_weights=True, vit_sd=None,
-                 max_len=1024, log=None, edit=False, llm_weight_format="fp16"):
+                 max_len=1024, log=None, edit=False, llm_weight_format="fp16", unet_weight_format="fp16"):
         """edit=True builds the SEED-X-Edit pipe (eval_img2edit_seed_x_edit.py): 8-channel conv_in UNet behind SDXLAdapterWithLatentImage and
         the VAE encoder for the source image.  llm_weight_format: "fp16" or "fp8_e4m3" (LlamaForCausalLM's weight_format: FP8 projection
-        weights with per-row scales, half the bytes per decode step)."""
+        weights with per-row scales, half the bytes per decode step).  unet_weight_format: "fp16" or "fp8_e4m3" (UNet2DConditionModel's
+        weight_format: the transformer-block projections run as FP8 GEMMs with per-row scales)."""
         log = log or (lambda *a: None)
         t0 = time.time()
         vit_cfg = dict(VIT_G if vit_cfg is None else vit_cfg)
@@ -59,7 +60,7 @@ class SeedXEngine:
             self.agent = ContinuousLVLM.from_pretrained(llm=self.llm, input_resampler=Resampler(8, D, heads_in, V),
                                                         output_resampler=Resampler(8, V, heads_out, D), add_patch_pos=True, vit_down=True)
             self.agent.load_state_dict(synth.agent_state_dict(D, V))
-            unet = UNet2DConditionModel(unet_cfg)
+            unet = UNet2DConditionModel(unet_cfg, weight_format=unet_weight_format)
             unet.load_state_dict(synth.unet_state_dict(unet_cfg))
             log(f"unet ready {time.time() - t0:.1f}s")
             self.vae = AutoencoderKL(vae_cfg)

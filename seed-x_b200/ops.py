@@ -53,7 +53,7 @@ def _ensure_workspace(device):
 
 def gemm(a, w, out=None, *, bias=None, bias_m=None, bias_g=None, bias_g_rows=0, residual=None, res_row_mod=0,
          act=ACT_NONE, gated=False, alpha=1.0, out_dtype=torch.float16, tile_n=0, ln=None, dynamic_b=False, row_part=None, col_part=None,
-         row_stats=None):
+         row_stats=None, a_scale=None, w_scale=None):
     """out[b,m,n] = epi(alpha * a[b,m,:] . w[(b,)n,:]).
 
     a: fp16 [M,K] or [B,M,K] (last dim contiguous); w: fp16 [N,K] or [B,N,K]; returns/updates out [.., M, N_out].
@@ -63,10 +63,19 @@ def gemm(a, w, out=None, *, bias=None, bias_m=None, bias_g=None, bias_g_rows=0, 
     row_part / col_part: fp32 outputs [N/32, M, 2] / [M/32, N, 2] receiving partial (sum, sum of squares) of the stored output per row chunk /
          per 32-row slab and column, for the LayerNorm / GroupNorm that reads this output next (see stats_buffers()).
     dynamic_b: w is an activation written by the kernel launched just before (default: weights, prefetched before the PDL wait).
+    a, w float8_e4m3fn (2-D only) with a_scale fp32 [M] and w_scale fp32 [N] (row m of the true a = a_scale[m] * a[m], likewise w): seedx_gemm_fp8,
+         whose epilogue scales the accumulator by a_scale[m] * w_scale[n] and then runs as above.
     """
-    _require_cuda(a, w, out, bias, residual)
+    _require_cuda(a, w, out, bias, residual, a_scale, w_scale)
     _ensure_workspace(a.device)
-    assert a.dtype == torch.float16 and w.dtype == torch.float16
+    fp8 = a.dtype == torch.float8_e4m3fn
+    if fp8:
+        if w.dtype != torch.float8_e4m3fn or a_scale is None or w_scale is None:
+            raise _lib.SeedxError("an FP8 gemm needs float8_e4m3fn a and w and both a_scale and w_scale")
+        for t, n in ((a_scale, a.shape[-2]), (w_scale, w.shape[-2])):
+            assert t.dtype == torch.float32 and t.is_contiguous() and t.numel() == n
+    else:
+        assert a.dtype == torch.float16 and w.dtype == torch.float16 and a_scale is None and w_scale is None
     assert a.stride(-1) == 1 and w.stride(-1) == 1
     batched = a.dim() == 3
     B = a.shape[0] if batched else 1
@@ -115,8 +124,29 @@ def gemm(a, w, out=None, *, bias=None, bias_m=None, bias_g=None, bias_g_rows=0, 
         assert row_part is not None and st.dtype == torch.float32 and st.numel() == 2 * M and tk.dtype == torch.int32 and tk.numel() >= M // 32
         g.row_stats_out, g.row_tickets, g.row_eps = st.data_ptr(), tk.data_ptr(), float(eps)
     g.b_dynamic = int(dynamic_b)
-    check(lib().seedx_gemm_f16(C.byref(g), _stream()), "seedx_gemm_f16")
+    if fp8:
+        check(lib().seedx_gemm_fp8(C.byref(g), _ptr(a_scale), _ptr(w_scale), _stream()), "seedx_gemm_fp8")
+    else:
+        check(lib().seedx_gemm_f16(C.byref(g), _stream()), "seedx_gemm_f16")
     return out
+
+
+def quant_rows_fp8(x, q=None, scale=None):
+    """Per-row FP8 quantisation of fp16 x [rows, cols] (row-strided view): scale[r] = amax|x[r]| / 448 (1 for a zero row), q = e4m3(x / scale)
+    -> (q float8_e4m3fn [rows, cols], scale fp32 [rows]); bit-identical to llm.quantize_fp8_rows(x.float()).  A default q is a view of a buffer
+    whose rows are padded to 16 bytes (the A operand of an FP8 gemm)."""
+    _require_cuda(x, q, scale)
+    assert x.dtype == torch.float16 and x.dim() == 2 and x.stride(1) == 1
+    rows, cols = x.shape
+    if q is None:
+        q = torch.empty((rows, (cols + 15) // 16 * 16), device=x.device, dtype=torch.float8_e4m3fn)[:, :cols]
+    if scale is None:
+        scale = torch.empty((rows,), device=x.device, dtype=torch.float32)
+    assert q.dtype == torch.float8_e4m3fn and q.shape == x.shape and q.stride(1) == 1
+    assert scale.dtype == torch.float32 and scale.is_contiguous() and scale.numel() == rows
+    check(lib().seedx_quant_rows_fp8(_ptr(x), _i64(x.stride(0)), _i64(rows), _i64(cols), _ptr(q), _i64(q.stride(0)), _ptr(scale), _stream()),
+          "seedx_quant_rows_fp8")
+    return q, scale
 
 
 def row_finalize(row_part, eps, out=None):

@@ -17,11 +17,13 @@ import torch
 
 from . import ops
 from ._lib import SeedxError
+from .llm import quantize_fp8_rows
 
 SDXL_UNET = dict(in_channels=4, out_channels=4, block_out_channels=(320, 640, 1280), layers_per_block=2,
                  down_attn=(False, True, True), transformer_layers=(1, 2, 10), heads=(5, 10, 20), cross_attention_dim=2048,
                  time_embed_dim=1280, addition_time_embed_dim=256, text_embed_dim=1280, groups=32)
 SDXL_VAE = dict(block_out_channels=(128, 256, 512, 512), layers_per_block=2, latent_channels=4, groups=32, scaling_factor=0.13025)
+UNET_WEIGHT_FORMATS = ("fp16", "fp8_e4m3")
 
 
 def _load_weights_dir(path):
@@ -247,8 +249,12 @@ class _Transformer:
     # halves the HBM traffic of the residual epilogues and LayerNorm reads; fp32 is available for parity experiments.
     stream_dtype = torch.float16
 
-    def __init__(self, sd, p, dev, depth, heads, reg=None):
+    def __init__(self, sd, p, dev, depth, heads, reg=None, fp8=False):
+        """fp8: every projection GEMM of the block runs as e4m3 x e4m3 (seedx_gemm_fp8) on per-row FP8 copies of the packed fp16 weights;
+        the fp16 weights stay resident (they are what the registry and the folding update) and the copies are re-derived from them in place
+        (requantize_fp8) whenever a checkpoint changes weights."""
         self.heads = heads
+        self.fp8 = fp8
         self.norm = (_f(sd[p + ".norm.weight"], dev), _f(sd[p + ".norm.bias"], dev))
         self.w_in, self.b_in = _h(sd[p + ".proj_in.weight"], dev), _f(sd[p + ".proj_in.bias"], dev)
         self.w_out, self.b_out = _h(sd[p + ".proj_out.weight"], dev), _f(sd[p + ".proj_out.bias"], dev)
@@ -293,6 +299,41 @@ class _Transformer:
                 reg.add(f"{b}.ff.net.0.proj.weight", ff1.w, keep(ff1.w), hook=lambda v, fl=ff1: fl.set_all(v))
                 reg.add(f"{b}.ff.net.0.proj.bias", ff1.raw_bias, keep(ff1.raw_bias), hook=lambda v, fl=ff1: fl.set_bias(v))
                 reg.add(f"{b}.ff.net.2.weight", blk["w_ff2"], hh), reg.add(f"{b}.ff.net.2.bias", blk["b_ff2"], ff)
+        # FP8 copies: name -> (packed fp16 source, q float8_e4m3fn, s fp32 per output row, colsum8 of a folded projection or None)
+        self.fp8_w = {}
+        if fp8:
+            for name, w16, folded in (("proj_in", self.w_in, False), ("proj_out", self.w_out, False)):
+                self.fp8_w[name] = self._fp8_copy(w16, folded)
+            for blk in self.blocks:
+                blk["fp8"] = {name: self._fp8_copy(w16, folded) for name, w16, folded in (
+                    ("attn1.qkv", blk["qkv"].w, True), ("attn1.to_out", blk["w_o1"], False), ("attn2.to_q", blk["q2"].w, True),
+                    ("attn2.to_out", blk["w_o2"], False), ("ff.net.0", blk["ff1"].w, True), ("ff.net.2", blk["w_ff2"], False))}
+
+    @staticmethod
+    def _fp8_rows(w16):
+        """(q, s, colsum8) of a packed fp16 weight.  colsum8[n] = s[n] * sum_k float(q[n, k]): the folded LayerNorm's mean correction must cancel
+        against the weights the MMA actually sums, the dequantized FP8 ones (as _FoldedLinear takes its colsum from the ROUNDED fp16 weights)."""
+        q, sc = quantize_fp8_rows(w16)
+        return q, sc, q.float().sum(dim=1) * sc
+
+    def _fp8_copy(self, w16, folded):
+        q, sc, cs = self._fp8_rows(w16)
+        return (w16, q, sc, cs if folded else None)
+
+    def fp8_slots(self):
+        """every FP8 copy of this transformer: (name, (fp16 source, q, s, colsum8 or None))"""
+        out = list(self.fp8_w.items())
+        for blk in self.blocks:
+            out += list(blk.get("fp8", {}).items())
+        return out
+
+    def requantize_fp8(self):
+        """re-derive every FP8 copy from its fp16 source, writing q, s and colsum8 in place (captured graphs keep their pointers)"""
+        for _, (w16, q, sc, cs) in self.fp8_slots():
+            nq, ns, ncs = self._fp8_rows(w16)
+            q.copy_(nq), sc.copy_(ns)
+            if cs is not None:
+                cs.copy_(ncs)
 
     def context_kv(self, ctx16):
         """cross-attention K/V of every block for a step-invariant context [B*T, ctx_dim] (hoisted out of the sampler loop)."""
@@ -329,7 +370,24 @@ class _Transformer:
             elif rs is None:
                 ops.row_finalize(rp, 1e-5, out=stats)
             return (stats, fl.colsum)
-        hs = ops.gemm(hn.view(M, c), self.w_in, bias=self.b_in, out_dtype=torch.float16, row_part=rp, row_stats=rs)
+        if self.fp8:
+            # every projection input is quantised per row right before its GEMM, into one scratch operand (the GEMM that reads it has finished
+            # before the next quantisation writes: each kernel waits for its predecessor)
+            a8 = torch.empty((M * 4 * c,), device=x.device, dtype=torch.float8_e4m3fn)
+            a8s = torch.empty((M,), device=x.device, dtype=torch.float32)
+
+        def proj(a, w16, w8, ln_fl=None, **kw):
+            """a . w^T through the fp16 GEMM, or through the FP8 GEMM on the quantised a and w8 = (fp16 source, q, s, colsum8)"""
+            if not self.fp8:
+                return ops.gemm(a, w16, ln=None if ln_fl is None else ln_of(ln_fl), **kw)
+            qa = a8[: a.shape[0] * a.shape[1]].view(a.shape[0], a.shape[1])
+            ops.quant_rows_fp8(a, q=qa, scale=a8s)
+            ln = None
+            if ln_fl is not None:
+                ln = (ln_of(ln_fl)[0], w8[3])
+            return ops.gemm(qa, w8[1], ln=ln, a_scale=a8s, w_scale=w8[2], **kw)
+        f8 = self.fp8_w
+        hs = proj(hn.view(M, c), self.w_in, f8.get("proj_in"), bias=self.b_in, out_dtype=torch.float16, row_part=rp, row_stats=rs)
         qkv = torch.empty((M, 3 * c), device=x.device, dtype=torch.float16)
         obuf = torch.empty((M, c), device=x.device, dtype=torch.float16)
         qbuf = torch.empty((M, c), device=x.device, dtype=torch.float16)
@@ -339,18 +397,19 @@ class _Transformer:
         ov = obuf.view(n, S, H, d).permute(0, 2, 1, 3)
         q2 = qbuf.view(n, S, H, d).permute(0, 2, 1, 3)
         for blk, kvb in zip(self.blocks, kv):
+            b8 = blk.get("fp8", {})
             # norm1 -> fused QKV, norm2 -> cross-attention q, norm3 -> GEGLU: the normalisation happens in the projection's epilogue
-            ops.gemm(hs, blk["qkv"].w, out=qkv, bias=blk["qkv"].bias, ln=ln_of(blk["qkv"]))
+            proj(hs, blk["qkv"].w, b8.get("attn1.qkv"), blk["qkv"], out=qkv, bias=blk["qkv"].bias)
             ops.attention(q1, k1, v1, ov, scale=scale)
-            ops.gemm(obuf, blk["w_o1"], out=hs, bias=blk["b_o1"], residual=hs, row_part=rp, row_stats=rs)
-            ops.gemm(hs, blk["q2"].w, out=qbuf, bias=blk["q2"].bias, ln=ln_of(blk["q2"]))
+            proj(obuf, blk["w_o1"], b8.get("attn1.to_out"), out=hs, bias=blk["b_o1"], residual=hs, row_part=rp, row_stats=rs)
+            proj(hs, blk["q2"].w, b8.get("attn2.to_q"), blk["q2"], out=qbuf, bias=blk["q2"].bias)
             kv5 = kvb.view(n, n_ctx, 2, H, d)
             ops.attention(q2, kv5[:, :, 0].permute(0, 2, 1, 3), kv5[:, :, 1].permute(0, 2, 1, 3), ov, scale=scale)
-            ops.gemm(obuf, blk["w_o2"], out=hs, bias=blk["b_o2"], residual=hs, row_part=rp, row_stats=rs)
-            ops.gemm(hs, blk["ff1"].w, out=fbuf, bias=blk["ff1"].bias, act=ops.ACT_GELU, gated=True, ln=ln_of(blk["ff1"]))
-            ops.gemm(fbuf, blk["w_ff2"], out=hs, bias=blk["b_ff2"], residual=hs, row_part=rp, row_stats=rs)
+            proj(obuf, blk["w_o2"], b8.get("attn2.to_out"), out=hs, bias=blk["b_o2"], residual=hs, row_part=rp, row_stats=rs)
+            proj(hs, blk["ff1"].w, b8.get("ff.net.0"), blk["ff1"], out=fbuf, bias=blk["ff1"].bias, act=ops.ACT_GELU, gated=True)
+            proj(fbuf, blk["w_ff2"], b8.get("ff.net.2"), out=hs, bias=blk["b_ff2"], residual=hs, row_part=rp, row_stats=rs)
         po = _new_col_part(n, h, w, c, x.device)
-        return _tag(ops.gemm(hs, self.w_out, bias=self.b_out, residual=x.view(M, c), col_part=po).view(n, h, w, c), po)
+        return _tag(proj(hs, self.w_out, f8.get("proj_out"), bias=self.b_out, residual=x.view(M, c), col_part=po).view(n, h, w, c), po)
 
 
 # diffusers name of the block above: src/inference/eval_img2edit_seed_x_edit.py:8 imports it (and never instantiates it)
@@ -375,7 +434,13 @@ def pack_conv_dense(w, dev):
 class UNet2DConditionModel:
     """SDXL UNet (forward only). ``cfg`` follows SDXL_UNET; in_channels 8 = the edit variant (adapter_modules.py:183-198)."""
 
-    def __init__(self, cfg=None, device="cuda"):
+    def __init__(self, cfg=None, device="cuda", weight_format="fp16"):
+        """weight_format="fp8_e4m3": the projection GEMMs of every transformer block (proj_in, fused QKV, attn1.to_out, attn2.to_q,
+        attn2.to_out, GEGLU ff.net.0, ff.net.2, proj_out) run as e4m3 x e4m3 with per-row scales on both operands; everything else (convs,
+        attention, the hoisted cross-attention K/V, embeddings) stays fp16.  The fp16 weights stay resident beside the FP8 copies."""
+        if weight_format not in UNET_WEIGHT_FORMATS:
+            raise SeedxError(f"weight_format {weight_format!r}: expected one of {UNET_WEIGHT_FORMATS}")
+        self.weight_format = weight_format
         self.cfg = dict(SDXL_UNET if cfg is None else cfg)
         self.device = torch.device(device)
         self.dtype = torch.float16
@@ -394,7 +459,7 @@ class UNet2DConditionModel:
                        transformer_layers=tuple(c["transformer_layers_per_block"]), heads=tuple(c["attention_head_dim"]),
                        cross_attention_dim=c["cross_attention_dim"], addition_time_embed_dim=c["addition_time_embed_dim"],
                        down_attn=tuple("CrossAttn" in t for t in c["down_block_types"]))
-        m = cls(cfg, device=kw.get("device", "cuda"))
+        m = cls(cfg, device=kw.get("device", "cuda"), weight_format=kw.get("weight_format", "fp16"))
         m.load_state_dict(_load_weights_dir(d))
         return m
 
@@ -403,6 +468,9 @@ class UNet2DConditionModel:
 
     def eval(self):
         return self
+
+    def transformers(self):
+        return [t for b in self.down for t in b["att"]] + [self.mid["att"]] + [t for b in self.up for t in b["att"]]
 
     def state_shape_in_channels(self):
         return self.cfg["in_channels"]
@@ -423,6 +491,9 @@ class UNet2DConditionModel:
         for k in sorted((k for k in sd if k in self._reg.slots), key=lambda k: (0 if ".norm" in k else 1)):
             self._reg.update(k, sd[k])
         self._reg.finish()
+        if self.weight_format == "fp8_e4m3":
+            for t in self.transformers():
+                t.requantize_fp8()
         return unexpected
 
     def load_state_dict(self, sd, strict=False):
@@ -433,6 +504,7 @@ class UNet2DConditionModel:
         boc = cfg["block_out_channels"]
         nb = len(boc)
         reg = self._reg = _ParamRegistry()
+        fp8 = self.weight_format == "fp8_e4m3"
         cin = sd["conv_in.weight"].shape[1]
         self.cfg["in_channels"] = cin
         # widths the checkpoint itself fixes (diffusers: time_embed_dim = 4*block_out_channels[0], projection_class_embeddings_input_dim)
@@ -456,14 +528,14 @@ class UNet2DConditionModel:
             for j in range(cfg["layers_per_block"]):
                 blk["res"].append(_Resnet(sd, f"down_blocks.{i}.resnets.{j}", dev, 1e-5, reg))
                 if cfg["down_attn"][i]:
-                    blk["att"].append(_Transformer(sd, f"down_blocks.{i}.attentions.{j}", dev, cfg["transformer_layers"][i], cfg["heads"][i], reg))
+                    blk["att"].append(_Transformer(sd, f"down_blocks.{i}.attentions.{j}", dev, cfg["transformer_layers"][i], cfg["heads"][i], reg, fp8))
             if i < nb - 1:
                 p = f"down_blocks.{i}.downsamplers.0.conv"
                 blk["ds"] = (pack_conv_dense(sd[p + ".weight"], dev), _f(sd[p + ".bias"], dev))
                 reg.add(p + ".weight", blk["ds"][0], lambda t: pack_conv_dense(t, dev)), reg.add(p + ".bias", blk["ds"][1], ff)
             self.down.append(blk)
         self.mid = dict(r0=_Resnet(sd, "mid_block.resnets.0", dev, 1e-5, reg),
-                        att=_Transformer(sd, "mid_block.attentions.0", dev, cfg["transformer_layers"][-1], cfg["heads"][-1], reg),
+                        att=_Transformer(sd, "mid_block.attentions.0", dev, cfg["transformer_layers"][-1], cfg["heads"][-1], reg, fp8),
                         r1=_Resnet(sd, "mid_block.resnets.1", dev, 1e-5, reg))
         for i in range(nb):
             r = nb - 1 - i
@@ -471,7 +543,7 @@ class UNet2DConditionModel:
             for j in range(cfg["layers_per_block"] + 1):
                 blk["res"].append(_Resnet(sd, f"up_blocks.{i}.resnets.{j}", dev, 1e-5, reg))
                 if cfg["down_attn"][r]:
-                    blk["att"].append(_Transformer(sd, f"up_blocks.{i}.attentions.{j}", dev, cfg["transformer_layers"][r], cfg["heads"][r], reg))
+                    blk["att"].append(_Transformer(sd, f"up_blocks.{i}.attentions.{j}", dev, cfg["transformer_layers"][r], cfg["heads"][r], reg, fp8))
             if i < nb - 1:
                 p = f"up_blocks.{i}.upsamplers.0.conv"
                 blk["us"] = (pack_conv(sd[p + ".weight"], dev), _f(sd[p + ".bias"], dev))
