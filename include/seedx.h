@@ -140,6 +140,21 @@ int seedx_gemm_fp8(const seedx_gemm_args* args, const float* a_scale, const floa
  * q[r, c] = e4m3_rn(clamp(x[r, c] / scale[r], -448, 448)) with IEEE division, written to q (e4m3, row stride ldq bytes).  One read of the row,
  * 16-byte loads and stores.  Requires ldx % 8 == 0, ldq % 16 == 0, 16-byte aligned x and q, cols <= 8192.  Feeds the A operand of seedx_gemm_fp8. */
 int seedx_quant_rows_fp8(const void* x, int64_t ldx, int64_t rows, int64_t cols, void* q, int64_t ldq, float* scale, void* stream);
+/* The implicit-GEMM conv of seedx_gemm_f16 on FP8 operands: A is the NHWC e4m3 image [conv_n, conv_h, conv_w, conv_c] with one fp32 scale per
+ * IMAGE (a_scale[conv_n]: a scale constant over K is the only one the conv sum can carry, and no image's quantisation depends on the rest of the
+ * batch); B is e4m3 [N, taps*taps*roundup(C,128)] (k = (kh*taps + kw)*Cpad + c, zero channel padding) with one fp32 scale per output channel.
+ * Each 128-element k-block is summed by the MMAs from zero and then added into an fp32 accumulator, so long K (up to 23 040 for the UNet's
+ * 3x3 convs) keeps fp32 accuracy.  epilogue: x = (acc * a_scale[m / (H*W)]) * b_scale[n], then exactly the seedx_gemm_f16 conv epilogue
+ * (alpha, bias_n, per-image bias_g, activation, residual, store, col_part).  Rejected (error, nothing launched): a non-conv call, batch != 1,
+ * a NULL scale, C % 16 != 0, K != taps^2 * roundup(C,128), tile_n other than 0 (auto) / 64 / 128 / 160, and every image geometry the fp16 conv
+ * rejects.  Single-CTA tiles, data-parallel schedule; seedx_gemm_last_config reports it like any other launch. */
+int seedx_conv_fp8(const seedx_gemm_args* args, const float* a_scale, const float* b_scale, void* stream);
+/* Per-image FP8 quantisation of a contiguous fp16 tensor seen as [n, per_image] (an NHWC map, one row per image): scale[i] = amax |x[i, :]| / 448
+ * (1 for an all-zero image) and q[i, :] = e4m3_rn(clamp(x[i, :] / scale[i], -448, 448)) with IEEE division, q contiguous e4m3.  Two launches
+ * (per-chunk maxima into ws, then the per-image maximum and the conversion), deterministic.  ws: seedx_quant_images_fp8_ws_bytes(n, per_image)
+ * bytes, no initial contents.  Requires per_image % 16 == 0, 16-byte aligned x and q, n <= 65535.  Feeds the A operand of seedx_conv_fp8. */
+int seedx_quant_images_fp8(const void* x, int64_t n, int64_t per_image, void* q, float* scale, void* ws, void* stream);
+int64_t seedx_quant_images_fp8_ws_bytes(int64_t n, int64_t per_image);
 
 
 /* ------------------------------------------------------------------------------------------------

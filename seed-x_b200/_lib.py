@@ -52,6 +52,7 @@ def lib():
         _lib.seedx_last_error.restype = C.c_char_p
         _lib.seedx_launch_count.restype = C.c_int64
         _lib.seedx_groupnorm_ws_bytes.restype = C.c_int64
+        _lib.seedx_quant_images_fp8_ws_bytes.restype = C.c_int64
         _lib.seedx_abi_version.restype = C.c_int
         if "SEEDX_GEMM_CLUSTER" in os.environ:      # experiment switch: 0 = single-CTA tiles, 1 = auto, 2 = CTA pairs whenever legal
             _lib.seedx_gemm_set_cluster(int(os.environ["SEEDX_GEMM_CLUSTER"]))

@@ -126,6 +126,93 @@ quant_rows_fp8_kernel(const __half* __restrict__ x, long long ldx, long long row
   if (tcol < cols) qr[tcol] = (uint8_t)f32x2_to_e4m3x2(fp8_quant_val(tv, s), 0.f);
 }
 
+// Per-image FP8 (e4m3) quantisation of a contiguous fp16 tensor seen as [n, per_image] (an NHWC activation, one row per image): the A operand
+// of seedx_conv_fp8.  An image (up to 128 x 128 x 960 values) is far more than a warp's registers hold, so it takes two launches over
+// (chunk, image), QI_CHUNK values per CTA:
+//   1. quant_images_amax_kernel: the |x| maximum of every chunk -> ws[image][chunk];
+//   2. quant_images_fp8_kernel: every CTA reduces its image's chunk maxima (a maximum is order-free: deterministic, with no atomics and no
+//      zero fill), s = amax / 448 (1 for an all-zero image), and converts its chunk, q = e4m3_rn(clamp(x / s, +-448)) with IEEE division.
+// A thread holds QI_UNITS units of 16 values: two 16-byte loads and one 16-byte store each.
+constexpr int QI_THREADS = 256;
+constexpr int QI_UNITS = 2;
+constexpr int QI_CHUNK_UNITS = QI_THREADS * QI_UNITS;
+constexpr int QI_CHUNK = 16 * QI_CHUNK_UNITS;   // 8192 values
+
+SEEDX_DEVINL float block_max_qi(float v, float* sm) {   // every thread gets the CTA's maximum
+  v = warp_max(v);
+  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = v;
+  __syncthreads();
+  return warp_max((threadIdx.x & 31) < QI_THREADS / 32 ? sm[threadIdx.x & 31] : 0.f);
+}
+
+__global__ void __launch_bounds__(QI_THREADS)
+quant_images_amax_kernel(const __half* __restrict__ x, long long per_image, float* __restrict__ ws) {
+  __shared__ float sm[QI_THREADS / 32];
+  pdl_wait();
+  pdl_trigger();
+  const long long units = per_image >> 4;
+  const __half* xi = x + (long long)blockIdx.y * per_image;
+  __half2 mx = __float2half2_rn(0.f);
+#pragma unroll
+  for (int j = 0; j < QI_UNITS; ++j) {
+    const long long u = (long long)blockIdx.x * QI_CHUNK_UNITS + j * QI_THREADS + threadIdx.x;
+    if (u < units) {
+      const uint4 a = __ldg((const uint4*)(xi + 16 * u)), b = __ldg((const uint4*)(xi + 16 * u + 8));
+      const __half2* h0 = (const __half2*)&a;
+      const __half2* h1 = (const __half2*)&b;
+#pragma unroll
+      for (int e = 0; e < 4; ++e) mx = __hmax2(mx, __hmax2(__habs2(h0[e]), __habs2(h1[e])));
+    }
+  }
+  const float amax = block_max_qi(fmaxf(__low2float(mx), __high2float(mx)), sm);
+  if (threadIdx.x == 0) ws[(long long)blockIdx.y * gridDim.x + blockIdx.x] = amax;
+}
+
+__global__ void __launch_bounds__(QI_THREADS)
+quant_images_fp8_kernel(const __half* __restrict__ x, long long per_image, const float* __restrict__ ws, uint8_t* __restrict__ q,
+                        float* __restrict__ scale) {
+  __shared__ float sm[QI_THREADS / 32];
+  pdl_wait();                               // the chunk maxima of launch 1
+  pdl_trigger();
+  const long long units = per_image >> 4;
+  const long long base = (long long)blockIdx.y * per_image;
+  uint4 v[QI_UNITS][2];
+#pragma unroll
+  for (int j = 0; j < QI_UNITS; ++j) {
+    const long long u = (long long)blockIdx.x * QI_CHUNK_UNITS + j * QI_THREADS + threadIdx.x;
+    if (u < units) {
+      v[j][0] = __ldg((const uint4*)(x + base + 16 * u));
+      v[j][1] = __ldg((const uint4*)(x + base + 16 * u + 8));
+    }
+  }
+  const int chunks = (int)gridDim.x;
+  float m = 0.f;
+  for (int i = threadIdx.x; i < chunks; i += QI_THREADS) m = fmaxf(m, __ldcg(ws + (long long)blockIdx.y * chunks + i));
+  const float amax = block_max_qi(m, sm);
+  float s = __fdiv_rn(amax, 448.f);
+  s = s > 0.f ? s : 1.f;
+  if (blockIdx.x == 0 && threadIdx.x == 0) scale[blockIdx.y] = s;
+#pragma unroll
+  for (int j = 0; j < QI_UNITS; ++j) {
+    const long long u = (long long)blockIdx.x * QI_CHUNK_UNITS + j * QI_THREADS + threadIdx.x;
+    if (u < units) {
+      uint32_t o[4];
+#pragma unroll
+      for (int w = 0; w < 4; ++w) {   // 4 output words of 4 values: halves 2w, 2w+1 of the 16
+        const uint4& src = v[j][w >> 1];
+        const uint32_t a0 = (w & 1) ? src.z : src.x, a1 = (w & 1) ? src.w : src.y;
+        const float2 f0 = __half22float2(*(const __half2*)&a0), f1 = __half22float2(*(const __half2*)&a1);
+        const uint32_t lo = f32x2_to_e4m3x2(fp8_quant_val(f0.x, s), fp8_quant_val(f0.y, s));
+        const uint32_t hi = f32x2_to_e4m3x2(fp8_quant_val(f1.x, s), fp8_quant_val(f1.y, s));
+        o[w] = lo | (hi << 16);
+      }
+      *(uint4*)(q + base + 16 * u) = make_uint4(o[0], o[1], o[2], o[3]);
+    }
+  }
+}
+
+static int64_t quant_images_chunks(int64_t per_image) { return (per_image + QI_CHUNK - 1) / QI_CHUNK; }
+
 // im2col for strided convs on NHWC fp16 (k x k taps, stride s, pad_before on top/left, zero fill), 8 channels / thread
 __global__ void im2col_nhwc_kernel(const __half* __restrict__ x, int n, int h, int w, int c, int k, int stride, int pad, int ho, int wo,
                                    __half* __restrict__ out) {
@@ -377,6 +464,26 @@ extern "C" int seedx_quant_rows_fp8(const void* x, int64_t ldx, int64_t rows, in
   else launch_k(quant_rows_fp8_kernel<16>, grid, 128, 0, st, xp, (long long)ldx, (long long)rows, (int)cols, qp, (long long)ldq, scale);
   count_launch();
   return check_cuda(cudaGetLastError(), "quant_rows_fp8 launch");
+}
+
+extern "C" int64_t seedx_quant_images_fp8_ws_bytes(int64_t n, int64_t per_image) {
+  if (n <= 0 || per_image <= 0) return 0;
+  return n * quant_images_chunks(per_image) * (int64_t)sizeof(float);
+}
+
+extern "C" int seedx_quant_images_fp8(const void* x, int64_t n, int64_t per_image, void* q, float* scale, void* ws, void* stream) {
+  SEEDX_REQUIRE(x && q && scale && ws, "seedx_quant_images_fp8: null pointer");
+  SEEDX_REQUIRE(n > 0 && n <= 65535 && per_image > 0 && per_image % 16 == 0, "seedx_quant_images_fp8: n=%lld per_image=%lld (1 <= n <= 65535, per_image %% 16 == 0)",
+                (long long)n, (long long)per_image);
+  SEEDX_REQUIRE((uintptr_t)x % 16 == 0 && (uintptr_t)q % 16 == 0 && (uintptr_t)ws % 4 == 0, "seedx_quant_images_fp8: x and q must be 16-byte aligned");
+  const dim3 grid((unsigned)quant_images_chunks(per_image), (unsigned)n);
+  cudaStream_t st = (cudaStream_t)stream;
+  launch_k(quant_images_amax_kernel, grid, QI_THREADS, 0, st, (const __half*)x, (long long)per_image, (float*)ws);
+  count_launch();
+  if (int e = check_cuda(cudaGetLastError(), "quant_images_amax launch")) return e;
+  launch_k(quant_images_fp8_kernel, grid, QI_THREADS, 0, st, (const __half*)x, (long long)per_image, (const float*)ws, (uint8_t*)q, scale);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "quant_images_fp8 launch");
 }
 
 extern "C" int seedx_avgpool_tokens(const void* x, int dtype, int64_t n, int64_t t, int64_t c, int64_t k, void* out, void* stream) {

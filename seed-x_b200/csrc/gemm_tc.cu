@@ -149,14 +149,18 @@ SEEDX_DEVINL bool seg_next(const GemmParams& p, SegState& s, int n_clusters, int
 // 128 rows of A and HALF of the B tile, which TMA multicasts into both CTAs' shared memory: each SM fetches a quarter fewer operand bytes from L2.
 // A stage of a CTA is refilled only when the consumers of BOTH CTAs have released it (the peer writes into it), so every consumer warpgroup
 // arrives on the `empty` barriers of both CTAs.
-// TE = operand element type: __half, or __nv_fp8_e4m3 (single CTA, data-parallel, plain GEMM only: the host never instantiates FP8 with CL = 2,
-// stream-K or conv mode).  Every FP8 difference is under `if constexpr`, so the fp16 kernels are the same code with or without it.
-template <int BN, int CL, bool SK, typename TE = __half>
+// TE = operand element type: __half, or __nv_fp8_e4m3 (single CTA, data-parallel, batch 1 only: the host never instantiates FP8 with CL = 2 or
+// stream-K).  Every FP8 difference is under `if constexpr`, so the fp16 kernels are the same code with or without it.
+// CONV8 = the FP8 implicit-GEMM conv (seedx_conv_fp8; TE = e4m3, conv mode): the A window advances 128 channels per stage, every 128-element
+// k-block is accumulated by its own MMAs from zero and then added into the fp32 accumulator (promotion: the FP8 wgmma does not keep full fp32
+// over long K), and row m takes the scale of its image, a_scale[m / (H*W)].  Only the FP8 conv instantiations set it.
+template <int BN, int CL, bool SK, typename TE = __half, bool CONV8 = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmD,
                const __grid_constant__ CUtensorMap tmR, const GemmParams p) {
   using Cfg = TileCfg<BN, CL>;
   constexpr bool FP8 = std::is_same<TE, __nv_fp8_e4m3>::value;
+  static_assert(!CONV8 || (FP8 && CL == 1 && !SK), "the FP8 conv is single-CTA, data-parallel");
   constexpr int KB = FP8 ? BK_FP8 : BK;   // K elements per stage (TMA box coordinate step)
   const int STAGES = p.stages;
   if (threadIdx.x == 0) GEMM_STAMP(0);
@@ -262,7 +266,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             const int cc = kb - tap * p.c_chunks;
             const int kh = tap / p.taps_w;
             const int kw = tap - kh * p.taps_w;
-            tma_load_4d(sa, &tmA, full_bar(stage), cc * BK, w0 + kw - p.pad, h0 + kh - p.pad, img);
+            tma_load_4d(sa, &tmA, full_bar(stage), cc * (CONV8 ? BK_FP8 : BK), w0 + kw - p.pad, h0 + kh - p.pad, img);
           } else {
             tma_load_3d(sa, &tmA, full_bar(stage), kb * KB, m_blk * BM, b);
           }
@@ -314,12 +318,37 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       // ---- main loop: the MMAs of k-block kb are in flight while the stage of kb-1 is released
       {
         int prev = -1;
+        if constexpr (CONV8) {
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        }
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(full_bar(stage), phase);
           if (first_seg && kb == kb0 && ew == 0 && lane == 0) GEMM_STAMP(3);
           const uint32_t sa = smem_base + stage * Cfg::STAGE_BYTES + (uint32_t)(wg * 64 * BK * 2);
           const uint64_t adesc = wgmma_desc_k_sw128(sa);
           const uint64_t bdesc = wgmma_desc_k_sw128(smem_base + stage * Cfg::STAGE_BYTES + A_STAGE_BYTES);
+          if constexpr (CONV8) {
+            // promotion: the four QGMMAs of this 128-element k-block sum into `blk` from zero (scale-d = 0 on the first), their result is
+            // waited for, the stage goes back to the producer and the block sum is added into the fp32 accumulator by the CUDA cores.
+            // The other consumer warpgroup's MMAs keep the tensor core busy meanwhile.
+            float blk[BN / 2];
+            wgmma_fence_regs<BN / 2>(blk);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < BK / 16; ++k) wgmma_ss_e4m3<BN>(blk, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), k != 0);
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs<BN / 2>(blk);
+            release(stage);
+#pragma unroll
+            for (int i = 0; i < BN / 2; ++i) acc[i] += blk[i];
+            if (++stage == STAGES) {
+              stage = 0;
+              phase ^= 1u;
+            }
+            continue;
+          }
           wgmma_fence_regs<BN / 2>(acc);
           wgmma_fence();
 #pragma unroll
@@ -378,7 +407,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
       const float bm = (p.bias_m != nullptr && row_ok) ? p.bias_m[row] : 0.f;
       float a_s = 1.f;                         // FP8: the scale of this lane's row of A
-      if constexpr (FP8) a_s = row_ok ? __ldg(p.a_scale + row) : 0.f;
+      if constexpr (CONV8) a_s = row_ok ? __ldg(p.a_scale + row / (p.conv_h * p.conv_w)) : 0.f;   // one scale per image (rows = pixels)
+      else if constexpr (FP8) a_s = row_ok ? __ldg(p.a_scale + row) : 0.f;
       float ln_rstd = 1.f, ln_nmr = 0.f;       // folded LayerNorm: x = rstd * acc + (-mean * rstd) * colsum[n]
       if (p.ln_stats != nullptr && row_ok) {
         float2 mr;
@@ -776,7 +806,7 @@ constexpr size_t SK_FLAG_BYTES = 16384;
 // what the most recent launch ran (seedx_gemm_last_config): tile width, cluster size, stream-K, TMA epilogue, vec_ok, pipeline stages
 static int g_gemm_last[6] = {0, 0, 0, 0, 0, 0};
 
-template <int BN, int CL, typename TE = __half>
+template <int BN, int CL, typename TE = __half, bool CONV8 = false>
 static int launch_gemm_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& td, const CUtensorMap& tr, const GemmParams& p_in,
                           cudaStream_t st) {
   using Cfg = TileCfg<BN, CL>;
@@ -785,8 +815,8 @@ static int launch_gemm_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CU
   constexpr bool kHasSK = (CL == 2) && (BN % 32 == 0) && (BN >= 128) && !kFP8;
   static bool attr_done = false;
   if (!attr_done) {
-    SEEDX_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, CL, false, TE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
-    if (kHasSK) SEEDX_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, CL, kHasSK, TE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
+    SEEDX_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, CL, false, TE, CONV8>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
+    if (kHasSK) SEEDX_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, CL, kHasSK, TE, CONV8>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT));
     attr_done = true;
   }
   GemmParams p = p_in;
@@ -804,7 +834,8 @@ static int launch_gemm_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CU
     p.stages = Cfg::stages_for(epi_bytes, tail_bytes);
   }
   if (p.stages < 2) {
-    set_error("%s: tile %dx%d does not fit in shared memory with %d B of epilogue staging", kFP8 ? "seedx_gemm_fp8" : "seedx_gemm_f16", BM * CL, BN, epi_bytes);
+    set_error("%s: tile %dx%d does not fit in shared memory with %d B of epilogue staging", CONV8 ? "seedx_conv_fp8" : (kFP8 ? "seedx_gemm_fp8" : "seedx_gemm_f16"),
+              BM * CL, BN, epi_bytes);
     return 5;
   }
   const int smem_bytes = Cfg::smem_for(p.stages, epi_bytes, tail_bytes);
@@ -820,7 +851,7 @@ static int launch_gemm_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CU
       qa[0].id = cudaLaunchAttributeClusterDimension;
       qa[0].val.clusterDim.x = CL, qa[0].val.clusterDim.y = 1, qa[0].val.clusterDim.z = 1;
       q.attrs = qa, q.numAttrs = 1;
-      SEEDX_CUDA(cudaOccupancyMaxActiveClusters(&occ_clusters, gemm_tc_kernel<BN, CL, false, TE>, &q));
+      SEEDX_CUDA(cudaOccupancyMaxActiveClusters(&occ_clusters, gemm_tc_kernel<BN, CL, false, TE, CONV8>, &q));
       occ_smem = smem_bytes;
     }
     if (occ_clusters > 0 && occ_clusters < max_clusters) max_clusters = occ_clusters;
@@ -857,8 +888,8 @@ static int launch_gemm_cl(const CUtensorMap& ta, const CUtensorMap& tb, const CU
   cfg.attrs = attr;
   cfg.numAttrs = pdl_enabled() ? 2 : 1;
   g_gemm_last[0] = BN, g_gemm_last[1] = CL, g_gemm_last[2] = p.stream_k, g_gemm_last[3] = p.tma_epi, g_gemm_last[4] = p.vec_ok, g_gemm_last[5] = p.stages;
-  const cudaError_t e = (kHasSK && p.stream_k) ? cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, CL, kHasSK, TE>, ta, tb, td, tr, p)
-                                               : cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, CL, false, TE>, ta, tb, td, tr, p);
+  const cudaError_t e = (kHasSK && p.stream_k) ? cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, CL, kHasSK, TE, CONV8>, ta, tb, td, tr, p)
+                                               : cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BN, CL, false, TE, CONV8>, ta, tb, td, tr, p);
   count_launch();
   return check_cuda(e != cudaSuccess ? e : cudaGetLastError(), "gemm_tc_kernel launch");
 }
@@ -895,13 +926,15 @@ struct TileRate {
 };
 static const TileRate kAutoTiles[] = {{128, 0.82}, {160, 0.78}, {192, 0.94}, {224, 0.73}, {256, 1.0}};
 
-static int choose_tile_n(int m_tiles, int N, int k_blocks, bool heavy_epilogue, bool only32) {
+// max_bn: the widest tile the caller has kernels for (the FP8 conv: 160, see kConv8Tiles)
+static int choose_tile_n(int m_tiles, int N, int k_blocks, bool heavy_epilogue, bool only32, int max_bn = 256) {
   const int sms = num_sms();
   double best = 1e30;
   int best_bn = 256;
   for (const TileRate& tr : kAutoTiles) {
     const int bn = tr.bn;
     if (only32 && bn % 32 != 0) continue;  // the TMA epilogue stores whole 32-column chunks
+    if (bn > max_bn) continue;
     const int n_blocks = (N + bn - 1) / bn;
     const long long tiles = (long long)m_tiles * n_blocks;
     // stream-K (cluster pairs forced, workspace present): a launch of more than one wave costs its fractional number of waves plus the partial-tile round trip
@@ -945,10 +978,15 @@ extern "C" int seedx_gemm_set_workspace(void* ptr, int64_t bytes) {
   return 0;
 }
 
-// seedx_gemm_f16 and seedx_gemm_fp8: one host path.  FP8 differs in the element size (1 byte), the K per stage (128), the tensor-map type and the
-// scales; it runs single-CTA, data-parallel, batch 1, plain GEMM only, at the widths the auto chooser returns (and 64).
-static int gemm_entry(const seedx_gemm_args* a, bool fp8, const float* a_scale, const float* b_scale, void* stream) {
-  const char* fn = fp8 ? "seedx_gemm_fp8" : "seedx_gemm_f16";
+// FP8 conv tile widths: the promoted accumulation holds a second BN/2-register accumulator per consumer thread, and wider tiles spill under
+// the 232-register consumer budget
+static const int kConv8Tiles[] = {64, 128, 160};
+
+// seedx_gemm_f16, seedx_gemm_fp8 and seedx_conv_fp8: one host path.  FP8 differs in the element size (1 byte), the K per stage (128), the
+// tensor-map type and the scales; it runs single-CTA, data-parallel, batch 1, at the widths the auto chooser returns (and 64).  conv8: the FP8
+// implicit-GEMM conv (per-image a_scale, promoted accumulation), at the widths of kConv8Tiles.
+static int gemm_entry(const seedx_gemm_args* a, bool fp8, bool conv8, const float* a_scale, const float* b_scale, void* stream) {
+  const char* fn = conv8 ? "seedx_conv_fp8" : (fp8 ? "seedx_gemm_fp8" : "seedx_gemm_f16");
   SEEDX_REQUIRE(a != nullptr, "%s: null args", fn);
   SEEDX_REQUIRE(a->A && a->B && a->D, "%s: null operand pointer", fn);
   SEEDX_REQUIRE(a->M > 0 && a->N > 0 && a->K > 0 && a->batch > 0, "%s: empty problem M=%lld N=%lld K=%lld", fn,
@@ -956,7 +994,14 @@ static int gemm_entry(const seedx_gemm_args* a, bool fp8, const float* a_scale, 
   const int es = fp8 ? 1 : 2;                 // operand element bytes
   const int kb_elems = fp8 ? BK_FP8 : BK;     // K elements per pipeline stage
   const int row_align = 16 / es;              // elements per 16 bytes: TMA rows start and end on 16-byte boundaries
-  if (fp8) {
+  if (conv8) {
+    SEEDX_REQUIRE(a->conv_taps_h > 0 && a->conv_taps_w > 0, "seedx_conv_fp8: not a conv call (conv_taps_h / conv_taps_w are 0)");
+    SEEDX_REQUIRE(a->batch == 1, "seedx_conv_fp8: batch=%lld, only batch 1 is supported", (long long)a->batch);
+    SEEDX_REQUIRE(a_scale != nullptr && b_scale != nullptr, "seedx_conv_fp8: a_scale and b_scale are required");
+    bool tile_ok = a->tile_n == 0;
+    for (int t : kConv8Tiles) tile_ok = tile_ok || a->tile_n == t;
+    SEEDX_REQUIRE(tile_ok, "seedx_conv_fp8: tile_n must be 0 (auto) or one of 64/128/160");
+  } else if (fp8) {
     SEEDX_REQUIRE(a->conv_taps_h == 0 && a->conv_taps_w == 0, "seedx_gemm_fp8: conv mode is not supported");
     SEEDX_REQUIRE(a->batch == 1, "seedx_gemm_fp8: batch=%lld, only batch 1 is supported", (long long)a->batch);
     SEEDX_REQUIRE(a_scale != nullptr && b_scale != nullptr, "seedx_gemm_fp8: a_scale and b_scale are required");
@@ -1000,6 +1045,7 @@ static int gemm_entry(const seedx_gemm_args* a, bool fp8, const float* a_scale, 
     if (bn == 0) bn = choose_tile_n(p.m_blocks * (int)a->batch, (int)a->N, p.k_blocks, a->act != SEEDX_ACT_NONE, tma_epi);
   } else {
     const int64_t C = a->conv_c, W = a->conv_w, H = a->conv_h, NI = a->conv_n;
+    if (conv8) SEEDX_REQUIRE(C % 16 == 0 && C > 0, "seedx_conv_fp8: channels must be a multiple of 16 (16-byte e4m3 pixels)");
     SEEDX_REQUIRE(C % 8 == 0 && C > 0, "seedx_gemm_f16(conv): channels must be a multiple of 8");
     SEEDX_REQUIRE(a->conv_taps_h == a->conv_taps_w && (a->conv_taps_h == 1 || a->conv_taps_h == 3),
                   "seedx_gemm_f16(conv): only 1x1 and 3x3 kernels");
@@ -1017,15 +1063,18 @@ static int gemm_entry(const seedx_gemm_args* a, bool fp8, const float* a_scale, 
       tw = 128, th = 1;
     }
     SEEDX_REQUIRE(a->M == NI * H * W, "seedx_gemm_f16(conv): M != n*h*w");
-    const int cchunks = (int)((C + BK - 1) / BK);
-    SEEDX_REQUIRE(a->K == (int64_t)a->conv_taps_h * a->conv_taps_w * cchunks * BK,
-                  "seedx_gemm_f16(conv): K=%lld must equal taps*roundup(C,64)=%lld", (long long)a->K,
-                  (long long)a->conv_taps_h * a->conv_taps_w * cchunks * BK);
+    const int cchunks = (int)((C + kb_elems - 1) / kb_elems);   // channel chunks of one stage: 64 fp16 or 128 e4m3 (128 bytes per pixel)
+    SEEDX_REQUIRE(a->K == (int64_t)a->conv_taps_h * a->conv_taps_w * cchunks * kb_elems,
+                  "%s: K=%lld must equal taps*roundup(C,%d)=%lld", conv8 ? fn : "seedx_gemm_f16(conv)", (long long)a->K, kb_elems,
+                  (long long)a->conv_taps_h * a->conv_taps_w * cchunks * kb_elems);
     uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)NI};
-    uint64_t strides[3] = {(uint64_t)C * 2, (uint64_t)W * C * 2, (uint64_t)H * W * C * 2};
-    if (bn == 0) bn = choose_tile_n((int)((a->M + BM - 1) / BM), (int)a->N, a->conv_taps_h * a->conv_taps_w * cchunks, a->act != SEEDX_ACT_NONE, tma_epi);
-    uint32_t box[4] = {BK, (uint32_t)tw, (uint32_t)th, (uint32_t)tn};
-    if (int e = encode_tmap(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, a->A, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))
+    uint64_t strides[3] = {(uint64_t)C * es, (uint64_t)W * C * es, (uint64_t)H * W * C * es};
+    if (bn == 0)
+      bn = choose_tile_n((int)((a->M + BM - 1) / BM), (int)a->N, a->conv_taps_h * a->conv_taps_w * cchunks, a->act != SEEDX_ACT_NONE, tma_epi,
+                         conv8 ? 160 : 256);
+    uint32_t box[4] = {(uint32_t)kb_elems, (uint32_t)tw, (uint32_t)th, (uint32_t)tn};
+    if (int e = encode_tmap(&ta, conv8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, a->A, dims, strides, box,
+                            CU_TENSOR_MAP_SWIZZLE_128B))
       return e;
     p.conv = 1;
     p.taps_w = a->conv_taps_w;
@@ -1137,6 +1186,13 @@ static int gemm_entry(const seedx_gemm_args* a, bool fp8, const float* a_scale, 
     }
   }
   cudaStream_t st = (cudaStream_t)stream;
+  if (conv8) {
+    switch (bn) {
+      case 64: return launch_gemm_cl<64, 1, __nv_fp8_e4m3, true>(ta, tb, td, tr, p, st);
+      case 128: return launch_gemm_cl<128, 1, __nv_fp8_e4m3, true>(ta, tb, td, tr, p, st);
+      default: return launch_gemm_cl<160, 1, __nv_fp8_e4m3, true>(ta, tb, td, tr, p, st);
+    }
+  }
   if (fp8) {
     switch (bn) {
       case 64: return launch_gemm_cl<64, 1, __nv_fp8_e4m3>(ta, tb, td, tr, p, st);
@@ -1161,8 +1217,12 @@ static int gemm_entry(const seedx_gemm_args* a, bool fp8, const float* a_scale, 
   }
 }
 
-extern "C" int seedx_gemm_f16(const seedx_gemm_args* a, void* stream) { return gemm_entry(a, false, nullptr, nullptr, stream); }
+extern "C" int seedx_gemm_f16(const seedx_gemm_args* a, void* stream) { return gemm_entry(a, false, false, nullptr, nullptr, stream); }
 
 extern "C" int seedx_gemm_fp8(const seedx_gemm_args* a, const float* a_scale, const float* b_scale, void* stream) {
-  return gemm_entry(a, true, a_scale, b_scale, stream);
+  return gemm_entry(a, true, false, a_scale, b_scale, stream);
+}
+
+extern "C" int seedx_conv_fp8(const seedx_gemm_args* a, const float* a_scale, const float* b_scale, void* stream) {
+  return gemm_entry(a, true, true, a_scale, b_scale, stream);
 }

@@ -24,8 +24,9 @@ class SeedXEngine:
                  max_len=1024, log=None, edit=False, llm_weight_format="fp16", unet_weight_format="fp16"):
         """edit=True builds the SEED-X-Edit pipe (eval_img2edit_seed_x_edit.py): 8-channel conv_in UNet behind SDXLAdapterWithLatentImage and
         the VAE encoder for the source image.  llm_weight_format: "fp16" or "fp8_e4m3" (LlamaForCausalLM's weight_format: FP8 projection
-        weights with per-row scales, half the bytes per decode step).  unet_weight_format: "fp16" or "fp8_e4m3" (UNet2DConditionModel's
-        weight_format: the transformer-block projections run as FP8 GEMMs with per-row scales)."""
+        weights with per-row scales, half the bytes per decode step).  unet_weight_format: "fp16", "fp8_e4m3" or "fp8_e4m3_conv"
+        (UNet2DConditionModel's weight_format: the transformer-block projections run as FP8 GEMMs with per-row scales; "fp8_e4m3_conv" also
+        runs the ResnetBlock2D and upsampler 3x3 convs as FP8 convs with per-image scales)."""
         log = log or (lambda *a: None)
         t0 = time.time()
         vit_cfg = dict(VIT_G if vit_cfg is None else vit_cfg)

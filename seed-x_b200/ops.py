@@ -149,6 +149,34 @@ def quant_rows_fp8(x, q=None, scale=None):
     return q, scale
 
 
+def quant_images_fp8(x, q=None, scale=None, ws=None):
+    """Per-image FP8 quantisation of a contiguous fp16 tensor x [n, ...] (an NHWC map): scale[i] = amax|x[i]| / 448 (1 for an all-zero image),
+    q = e4m3(x / scale[i]) -> (q float8_e4m3fn shaped like x, scale fp32 [n]); bit-identical to llm.quantize_fp8_rows(x.view(n, -1).float()).
+    The A operand of an FP8 conv2d_nhwc.  ws: scratch of the per-chunk maxima (quant_images_fp8_ws(...), a few KB), allocated per call
+    when not given."""
+    _require_cuda(x, q, scale)
+    assert x.dtype == torch.float16 and x.is_contiguous()
+    n = x.shape[0]
+    per_image = x.numel() // n
+    if q is None:
+        q = torch.empty(x.shape, device=x.device, dtype=torch.float8_e4m3fn)
+    if scale is None:
+        scale = torch.empty((n,), device=x.device, dtype=torch.float32)
+    assert q.dtype == torch.float8_e4m3fn and q.is_contiguous() and q.numel() == x.numel()
+    assert scale.dtype == torch.float32 and scale.is_contiguous() and scale.numel() == n
+    if ws is None:
+        ws = quant_images_fp8_ws(n, per_image, x.device)
+    assert ws.numel() * ws.element_size() >= lib().seedx_quant_images_fp8_ws_bytes(_i64(n), _i64(per_image))
+    check(lib().seedx_quant_images_fp8(_ptr(x), _i64(n), _i64(per_image), _ptr(q), _ptr(scale), _ptr(ws), _stream()), "seedx_quant_images_fp8")
+    return q, scale
+
+
+def quant_images_fp8_ws(n, per_image, device):
+    """scratch for quant_images_fp8 of n images of per_image values: one fp32 maximum per 8192-value chunk"""
+    nbytes = int(lib().seedx_quant_images_fp8_ws_bytes(_i64(n), _i64(per_image)))
+    return torch.empty(((nbytes + 3) // 4,), device=device, dtype=torch.float32)
+
+
 def row_finalize(row_part, eps, out=None):
     """(mean, rstd) per row from the row partials [cols/32, rows, 2] a producing GEMM emitted (gemm(..., row_part=...)) -> fp32 [rows, 2]"""
     _require_cuda(row_part, out)
@@ -182,12 +210,22 @@ def row_stats(x, eps, out=None):
 
 
 def conv2d_nhwc(x, w, out=None, *, taps=3, bias=None, bias_g=None, residual=None, act=ACT_NONE,
-                out_dtype=torch.float16, tile_n=0, alpha=1.0, col_part=None):
+                out_dtype=torch.float16, tile_n=0, alpha=1.0, col_part=None, a_scale=None, w_scale=None):
     """Stride-1 'same' convolution as an implicit GEMM.  x: fp16 NHWC [N,H,W,C]; w: fp16 [Cout, taps*taps*roundup(C,64)]
-    (k = (kh*taps+kw)*Cpad + c); out: NHWC [N,H,W,Cout].  bias_g: fp32 [N, Cout] added per image."""
-    _require_cuda(x, w, out, bias, residual)
+    (k = (kh*taps+kw)*Cpad + c); out: NHWC [N,H,W,Cout].  bias_g: fp32 [N, Cout] added per image.
+    x, w float8_e4m3fn with a_scale fp32 [N] (image i of the true x = a_scale[i] * x[i]) and w_scale fp32 [Cout], w [Cout, taps*taps*roundup(C,128)]:
+    seedx_conv_fp8, whose epilogue scales the accumulator by a_scale[image] * w_scale[n] and then runs as above."""
+    _require_cuda(x, w, out, bias, residual, a_scale, w_scale)
     _ensure_workspace(x.device)
-    assert x.dtype == torch.float16 and x.is_contiguous() and w.is_contiguous()
+    fp8 = x.dtype == torch.float8_e4m3fn
+    if fp8:
+        if w.dtype != torch.float8_e4m3fn or a_scale is None or w_scale is None:
+            raise _lib.SeedxError("an FP8 conv needs float8_e4m3fn x and w and both a_scale and w_scale")
+        for t, n_ in ((a_scale, x.shape[0]), (w_scale, w.shape[0])):
+            assert t.dtype == torch.float32 and t.is_contiguous() and t.numel() == n_
+    else:
+        assert x.dtype == torch.float16 and a_scale is None and w_scale is None
+    assert x.is_contiguous() and w.is_contiguous()
     n, h, wd, c = x.shape
     cout, K = w.shape
     if out is None:
@@ -215,7 +253,10 @@ def conv2d_nhwc(x, w, out=None, *, taps=3, bias=None, bias_g=None, residual=None
     g.conv_n, g.conv_h, g.conv_w, g.conv_c = n, h, wd, c
     g.tile_n = tile_n
     _set_parts(g, None, col_part, n * h * wd, cout)
-    check(lib().seedx_gemm_f16(C.byref(g), _stream()), "seedx_gemm_f16(conv)")
+    if fp8:
+        check(lib().seedx_conv_fp8(C.byref(g), _ptr(a_scale), _ptr(w_scale), _stream()), "seedx_conv_fp8")
+    else:
+        check(lib().seedx_gemm_f16(C.byref(g), _stream()), "seedx_gemm_f16(conv)")
     return out
 
 

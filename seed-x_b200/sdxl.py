@@ -23,7 +23,7 @@ SDXL_UNET = dict(in_channels=4, out_channels=4, block_out_channels=(320, 640, 12
                  down_attn=(False, True, True), transformer_layers=(1, 2, 10), heads=(5, 10, 20), cross_attention_dim=2048,
                  time_embed_dim=1280, addition_time_embed_dim=256, text_embed_dim=1280, groups=32)
 SDXL_VAE = dict(block_out_channels=(128, 256, 512, 512), layers_per_block=2, latent_channels=4, groups=32, scaling_factor=0.13025)
-UNET_WEIGHT_FORMATS = ("fp16", "fp8_e4m3")
+UNET_WEIGHT_FORMATS = ("fp16", "fp8_e4m3", "fp8_e4m3_conv")
 
 
 def _load_weights_dir(path):
@@ -80,6 +80,35 @@ def pack_conv(w, dev, cin_pad_to=None):
     wp = torch.zeros((cout, k, k, cpad), dtype=torch.float16, device=w.device)
     wp[..., :cin] = w.permute(0, 2, 3, 1).to(torch.float16)
     return wp.reshape(cout, k * k * cpad).to(dev).contiguous()
+
+
+def conv_fp8(w16, cin, taps=3):
+    """FP8 copy of a packed fp16 conv weight (pack_conv layout, Cpad = roundup(cin, 64)) for seedx_conv_fp8: (q, s) = quantize_fp8_rows(w16), the
+    scale per output channel, with q repacked to [Cout, taps*taps*roundup(cin, 128)] (the conv's 128-channel stages) and zero channel padding."""
+    cout = w16.shape[0]
+    q, sc = quantize_fp8_rows(w16)
+    c128 = (cin + 127) // 128 * 128
+    q8 = torch.zeros((cout, taps * taps, c128), dtype=torch.uint8, device=w16.device)
+    q8[..., :cin] = q.view(torch.uint8).view(cout, taps * taps, -1)[..., :cin]
+    return q8.view(cout, taps * taps * c128).view(torch.float8_e4m3fn), sc
+
+
+class _ConvFP8:
+    """FP8 copy of one packed fp16 3x3 conv weight (w16 stays resident and is what checkpoints update): q e4m3 [Cout, 9*roundup(cin, 128)] and
+    s fp32 [Cout], re-derived in place by requantize() so that captured graphs keep their pointers"""
+
+    def __init__(self, w16, cin):
+        self.w16, self.cin = w16, cin
+        self.q, self.s = conv_fp8(w16, cin)
+
+    def requantize(self):
+        q, sc = conv_fp8(self.w16, self.cin)
+        self.q.copy_(q), self.s.copy_(sc)
+
+    def __call__(self, x, **kw):
+        """the conv on fp16 NHWC x: x is quantised per image right before it (seedx_quant_images_fp8), then seedx_conv_fp8"""
+        qx, sx = ops.quant_images_fp8(x)
+        return ops.conv2d_nhwc(qx, self.q, a_scale=sx, w_scale=self.s, **kw)
 
 
 def pad_rows(w, b, nmin=8):
@@ -183,13 +212,18 @@ def _interleave_rows(w):
 
 
 class _Resnet:
-    def __init__(self, sd, p, dev, eps, reg=None):
+    def __init__(self, sd, p, dev, eps, reg=None, fp8=False):
+        """fp8: conv1 and conv2 run as FP8 convs (seedx_conv_fp8) on _ConvFP8 copies of the packed fp16 weights, their inputs quantised per image;
+        the shortcut and everything else stay fp16.  The VAE builds its blocks with fp8=False."""
         self.eps = eps
         self._sb = {}
         self.n1 = (_f(sd[p + ".norm1.weight"], dev), _f(sd[p + ".norm1.bias"], dev))
         self.n2 = (_f(sd[p + ".norm2.weight"], dev), _f(sd[p + ".norm2.bias"], dev))
         self.w1, self.b1 = pack_conv(sd[p + ".conv1.weight"], dev), _f(sd[p + ".conv1.bias"], dev)
         self.w2, self.b2 = pack_conv(sd[p + ".conv2.weight"], dev), _f(sd[p + ".conv2.bias"], dev)
+        self.fp8 = None
+        if fp8:
+            self.fp8 = dict(conv1=_ConvFP8(self.w1, sd[p + ".conv1.weight"].shape[1]), conv2=_ConvFP8(self.w2, sd[p + ".conv2.weight"].shape[1]))
         self.wt = self.bt = None
         if (p + ".time_emb_proj.weight") in sd:
             self.wt, self.bt = _h(sd[p + ".time_emb_proj.weight"], dev), _f(sd[p + ".time_emb_proj.bias"], dev)
@@ -233,7 +267,9 @@ class _Resnet:
             raise SeedxError("scaled-stream ResnetBlock2D with a time embedding is not used by any model")
         cout = self.w1.shape[0]
         p1 = _new_col_part(n, h, w, cout, x.device)            # norm2 statistics: emitted by conv1's epilogue
-        a = ops.conv2d_nhwc(a, self.w1, bias=b1, bias_g=tb, alpha=alpha, col_part=p1)
+        conv1 = self.fp8["conv1"] if self.fp8 else (lambda x, **kw: ops.conv2d_nhwc(x, self.w1, **kw))
+        conv2 = self.fp8["conv2"] if self.fp8 else (lambda x, **kw: ops.conv2d_nhwc(x, self.w2, **kw))
+        a = conv1(a, bias=b1, bias_g=tb, alpha=alpha, col_part=p1)
         a = ops.groupnorm_nhwc(a, self.n2[0], self.n2[1], eps, silu=True, groups=groups, stats_ws=ws, part1=p1)
         xin = raw if raw is not None else x
         if self.wsc is not None:
@@ -241,7 +277,7 @@ class _Resnet:
         else:
             sc = xin
         p2 = _new_col_part(n, h, w, cout, x.device)            # statistics of the block output for whichever GroupNorm reads it next
-        return _tag(ops.conv2d_nhwc(a, self.w2, bias=b2, residual=sc, alpha=alpha, col_part=p2), p2)
+        return _tag(conv2(a, bias=b2, residual=sc, alpha=alpha, col_part=p2), p2)
 
 
 class _Transformer:
@@ -437,7 +473,10 @@ class UNet2DConditionModel:
     def __init__(self, cfg=None, device="cuda", weight_format="fp16"):
         """weight_format="fp8_e4m3": the projection GEMMs of every transformer block (proj_in, fused QKV, attn1.to_out, attn2.to_q,
         attn2.to_out, GEGLU ff.net.0, ff.net.2, proj_out) run as e4m3 x e4m3 with per-row scales on both operands; everything else (convs,
-        attention, the hoisted cross-attention K/V, embeddings) stays fp16.  The fp16 weights stay resident beside the FP8 copies."""
+        attention, the hoisted cross-attention K/V, embeddings) stays fp16.  The fp16 weights stay resident beside the FP8 copies.
+        weight_format="fp8_e4m3_conv": all of that, and conv1 / conv2 of every ResnetBlock2D plus both upsampler convs run as FP8 convs with
+        one scale per image and per output channel (36 convs at SDXL size); conv_in, conv_out, the 1x1 shortcuts and the stride-2
+        downsamplers stay fp16."""
         if weight_format not in UNET_WEIGHT_FORMATS:
             raise SeedxError(f"weight_format {weight_format!r}: expected one of {UNET_WEIGHT_FORMATS}")
         self.weight_format = weight_format
@@ -472,6 +511,19 @@ class UNet2DConditionModel:
     def transformers(self):
         return [t for b in self.down for t in b["att"]] + [self.mid["att"]] + [t for b in self.up for t in b["att"]]
 
+    def conv_fp8_slots(self):
+        """every FP8 conv copy: (checkpoint prefix of the conv, _ConvFP8); empty unless weight_format="fp8_e4m3_conv" """
+        if not self._loaded:
+            return []
+        out = []
+        res = [(f"down_blocks.{i}.resnets.{j}", r) for i, b in enumerate(self.down) for j, r in enumerate(b["res"])]
+        res += [("mid_block.resnets.0", self.mid["r0"]), ("mid_block.resnets.1", self.mid["r1"])]
+        res += [(f"up_blocks.{i}.resnets.{j}", r) for i, b in enumerate(self.up) for j, r in enumerate(b["res"])]
+        for p, r in res:
+            out += [(f"{p}.{k}", c) for k, c in (r.fp8 or {}).items()]
+        out += [(f"up_blocks.{i}.upsamplers.0.conv", b["us8"]) for i, b in enumerate(self.up) if b.get("us8") is not None]
+        return out
+
     def state_shape_in_channels(self):
         return self.cfg["in_channels"]
 
@@ -491,9 +543,11 @@ class UNet2DConditionModel:
         for k in sorted((k for k in sd if k in self._reg.slots), key=lambda k: (0 if ".norm" in k else 1)):
             self._reg.update(k, sd[k])
         self._reg.finish()
-        if self.weight_format == "fp8_e4m3":
+        if self.weight_format in ("fp8_e4m3", "fp8_e4m3_conv"):
             for t in self.transformers():
                 t.requantize_fp8()
+        for _, c in self.conv_fp8_slots():
+            c.requantize()
         return unexpected
 
     def load_state_dict(self, sd, strict=False):
@@ -504,7 +558,8 @@ class UNet2DConditionModel:
         boc = cfg["block_out_channels"]
         nb = len(boc)
         reg = self._reg = _ParamRegistry()
-        fp8 = self.weight_format == "fp8_e4m3"
+        fp8 = self.weight_format in ("fp8_e4m3", "fp8_e4m3_conv")
+        conv8 = self.weight_format == "fp8_e4m3_conv"
         cin = sd["conv_in.weight"].shape[1]
         self.cfg["in_channels"] = cin
         # widths the checkpoint itself fixes (diffusers: time_embed_dim = 4*block_out_channels[0], projection_class_embeddings_input_dim)
@@ -526,7 +581,7 @@ class UNet2DConditionModel:
         for i in range(nb):
             blk = dict(res=[], att=[], ds=None)
             for j in range(cfg["layers_per_block"]):
-                blk["res"].append(_Resnet(sd, f"down_blocks.{i}.resnets.{j}", dev, 1e-5, reg))
+                blk["res"].append(_Resnet(sd, f"down_blocks.{i}.resnets.{j}", dev, 1e-5, reg, conv8))
                 if cfg["down_attn"][i]:
                     blk["att"].append(_Transformer(sd, f"down_blocks.{i}.attentions.{j}", dev, cfg["transformer_layers"][i], cfg["heads"][i], reg, fp8))
             if i < nb - 1:
@@ -534,20 +589,22 @@ class UNet2DConditionModel:
                 blk["ds"] = (pack_conv_dense(sd[p + ".weight"], dev), _f(sd[p + ".bias"], dev))
                 reg.add(p + ".weight", blk["ds"][0], lambda t: pack_conv_dense(t, dev)), reg.add(p + ".bias", blk["ds"][1], ff)
             self.down.append(blk)
-        self.mid = dict(r0=_Resnet(sd, "mid_block.resnets.0", dev, 1e-5, reg),
+        self.mid = dict(r0=_Resnet(sd, "mid_block.resnets.0", dev, 1e-5, reg, conv8),
                         att=_Transformer(sd, "mid_block.attentions.0", dev, cfg["transformer_layers"][-1], cfg["heads"][-1], reg, fp8),
-                        r1=_Resnet(sd, "mid_block.resnets.1", dev, 1e-5, reg))
+                        r1=_Resnet(sd, "mid_block.resnets.1", dev, 1e-5, reg, conv8))
         for i in range(nb):
             r = nb - 1 - i
-            blk = dict(res=[], att=[], us=None)
+            blk = dict(res=[], att=[], us=None, us8=None)
             for j in range(cfg["layers_per_block"] + 1):
-                blk["res"].append(_Resnet(sd, f"up_blocks.{i}.resnets.{j}", dev, 1e-5, reg))
+                blk["res"].append(_Resnet(sd, f"up_blocks.{i}.resnets.{j}", dev, 1e-5, reg, conv8))
                 if cfg["down_attn"][r]:
                     blk["att"].append(_Transformer(sd, f"up_blocks.{i}.attentions.{j}", dev, cfg["transformer_layers"][r], cfg["heads"][r], reg, fp8))
             if i < nb - 1:
                 p = f"up_blocks.{i}.upsamplers.0.conv"
                 blk["us"] = (pack_conv(sd[p + ".weight"], dev), _f(sd[p + ".bias"], dev))
                 reg.add(p + ".weight", blk["us"][0], lambda t: pack_conv(t, dev)), reg.add(p + ".bias", blk["us"][1], ff)
+                if conv8:
+                    blk["us8"] = _ConvFP8(blk["us"][0], sd[p + ".weight"].shape[1])
             self.up.append(blk)
         self.norm_out = (_f(sd["conv_norm_out.weight"], dev), _f(sd["conv_norm_out.bias"], dev))
         self.conv_out = (pack_conv(sd["conv_out.weight"], dev), _f(sd["conv_out.bias"], dev))
@@ -618,7 +675,10 @@ class UNet2DConditionModel:
             if blk["us"] is not None:
                 up = ops.upsample2x_nhwc(h)
                 pu = _new_col_part(up.shape[0], up.shape[1], up.shape[2], blk["us"][0].shape[0], self.device)
-                h = _tag(ops.conv2d_nhwc(up, blk["us"][0], bias=blk["us"][1], col_part=pu), pu)
+                if blk["us8"] is not None:
+                    h = _tag(blk["us8"](up, bias=blk["us"][1], col_part=pu), pu)
+                else:
+                    h = _tag(ops.conv2d_nhwc(up, blk["us"][0], bias=blk["us"][1], col_part=pu), pu)
         a = ops.groupnorm_nhwc(h, self.norm_out[0], self.norm_out[1], 1e-5, silu=True, groups=G, stats_ws=ws, part1=_part(h))
         return ops.conv2d_nhwc(a, self.conv_out[0], bias=self.conv_out[1], out_dtype=torch.float32, tile_n=64)
 
