@@ -252,6 +252,19 @@ int seedx_image_to_u8(const void* x, int x_dtype, int64_t pixels, int64_t ldc, u
  * eps == NULL: initialisation, x *= init_sigma (prepare_latents, pipeline...edit.py:474-488) */
 int seedx_cfg_euler_step(const float* eps, float* x, void* unet_in, int64_t batch, int64_t hw, int branches, float guidance,
                          float image_guidance, float sigma, float sigma_next, float init_sigma, void* stream);
+/* the same step for `slots` independent requests (continuous batching of the denoising loop), each at its own point of its own schedule:
+ *   state     int32 [slots][2]              (step index i, step count n) of each slot; a slot is live while i < n
+ *   sigmas    fp32  [slots][max_steps + 1]  its EulerDiscreteScheduler sigmas (entry n = 0), timesteps fp32 [slots][max_steps]
+ *   scalars   fp32  [slots][3]              guidance, image guidance, init_noise_sigma of its step count
+ *   t_dev     fp32  [branches * slots]      per-row UNet timestep, row br * slots + s; x / unet_in / eps as above with batch = slots
+ * eps != NULL: every live slot s combines with its own g, ig, sigma = sigmas[s][i], sigma_next = sigmas[s][i+1] (bit-identical to
+ * seedx_cfg_euler_step given the same fp32 values), writes x[s] and channels 0..3 of its unet_in rows, then i += 1 and, while i < n,
+ * t_dev rows = timesteps[s][i] (two launches: combine, then a one-CTA advance).  fresh_mask must be 0.
+ * eps == NULL: initialises exactly the slots whose bit is set in fresh_mask (!= 0): x = x * init_noise_sigma, unet_in scaled by sigmas[s][0],
+ * t_dev rows = timesteps[s][0]; state is not touched (one launch).
+ * Slots not live / not fresh keep x, unet_in and t_dev bytes.  1 <= slots <= 64, max_steps >= 1, branches 2 or 3; eps / unet_in 16-byte aligned. */
+int seedx_cfg_euler_slots(const float* eps, float* x, void* unet_in, float* t_dev, int32_t* state, const float* sigmas, const float* timesteps,
+                          const float* scalars, int64_t slots, int64_t hw, int branches, int64_t max_steps, uint64_t fresh_mask, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * LLaMA token loop (greedy decode of up to 8 sequences in lock-step; HBM-bound) and prefill glue.  Device-resident state:

@@ -361,6 +361,29 @@ __global__ void image_to_u8_kernel(const TI* __restrict__ x, long long pixels, i
 //   unet_in: fp16 NHWC [nb*B, HW, 8]; channels 0..3 <- x_new / sqrt(sigma_next^2 + 1) for every branch
 //   mode 2 (t2i, branches [uncond, text])   : e = e_u + g (e_t - e_u)                       (adapter_modules.py:156-167 -> diffusers SDXL pipeline)
 //   mode 3 (edit, branches [text, image, uncond]): sigma-space combine, pipeline_stable_diffusion_xl_t2i_edit.py:928-950
+// The per-element arithmetic lives in cfg_euler_update / cfg_euler_input, shared with cfg_euler_slots_kernel: a slot of the continuous batcher
+// gets the bits of this kernel given the same fp32 sigmas and guidance.  eps_at(br) returns the branch-br eps value of the element.
+template <typename EpsAt>
+SEEDX_DEVINL float cfg_euler_update(const EpsAt& eps_at, float xv, int mode, float g, float ig, float sigma, float sigma_next) {
+  float e;
+  if (mode == 2) {
+    const float eu = eps_at(0);
+    const float et = eps_at(1);
+    e = eu + g * (et - eu);
+  } else {
+    const float et = xv - sigma * eps_at(0);
+    const float ei = xv - sigma * eps_at(1);
+    const float eu = xv - sigma * eps_at(2);
+    const float c = eu + g * (et - ei) + ig * (ei - eu);
+    e = (c - xv) / (-sigma);
+  }
+  const float x0 = xv - sigma * e;
+  const float d = (xv - x0) / sigma;
+  return xv + d * (sigma_next - sigma);
+}
+
+SEEDX_DEVINL __half cfg_euler_input(float xn, float sigma_next) { return __float2half_rn(xn * rsqrtf(sigma_next * sigma_next + 1.f)); }
+
 __global__ void cfg_euler_kernel(const float* __restrict__ eps, float* __restrict__ x, __half* __restrict__ unet_in, int B, int hw, int mode,
                                  float g, float ig, float sigma, float sigma_next, float init_sigma) {
   pdl_wait();
@@ -377,26 +400,83 @@ __global__ void cfg_euler_kernel(const float* __restrict__ eps, float* __restric
     if (eps == nullptr) {
       xn = xv * init_sigma;
     } else {
-      float e;
-      if (mode == 2) {
-        const float eu = eps[(((long long)(0 * B + b)) * hw + p) * 4 + ch];
-        const float et = eps[(((long long)(1 * B + b)) * hw + p) * 4 + ch];
-        e = eu + g * (et - eu);
-      } else {
-        const float et = xv - sigma * eps[(((long long)(0 * B + b)) * hw + p) * 4 + ch];
-        const float ei = xv - sigma * eps[(((long long)(1 * B + b)) * hw + p) * 4 + ch];
-        const float eu = xv - sigma * eps[(((long long)(2 * B + b)) * hw + p) * 4 + ch];
-        const float c = eu + g * (et - ei) + ig * (ei - eu);
-        e = (c - xv) / (-sigma);
-      }
-      const float x0 = xv - sigma * e;
-      const float d = (xv - x0) / sigma;
-      xn = xv + d * (sigma_next - sigma);
+      xn = cfg_euler_update([&](int br) { return eps[(((long long)(br * B + b)) * hw + p) * 4 + ch]; }, xv, mode, g, ig, sigma, sigma_next);
     }
     x[xi] = xn;
-    const __half s = __float2half_rn(xn * rsqrtf(sigma_next * sigma_next + 1.f));
+    const __half s = cfg_euler_input(xn, sigma_next);
     for (int br = 0; br < mode; ++br) unet_in[(((long long)(br * B + b)) * hw + p) * 8 + ch] = s;
   }
+}
+
+// The same step for S independent request slots (seedx_b200.serving.DenoiseBatcher), every slot at its own point of its own schedule:
+//   state   int32 [S][2]         (step index i, step count n); slot s is live while i < n
+//   sig     fp32  [S][max_steps+1] its sigmas (trailing 0), ts fp32 [S][max_steps] its timesteps, scal fp32 [S][3] (g, ig, init_noise_sigma)
+// One thread per latent pixel: the 4 channels of a branch's eps are one 16-byte load, the 4 fp16 inputs one 8-byte store.  Slots that are
+// not live (eps != NULL) / not in fresh_mask (eps == NULL) are skipped: their x, unet_in and t_dev rows keep their bytes.
+// eps == NULL: initialisation of the fresh slots, x = noise * init_sigma[s], inputs scaled by sig[s][0], t_dev rows = ts[s][0].
+// This kernel only reads state; the step index is advanced by cfg_euler_slots_advance_kernel, a separate launch that starts its work after
+// every CTA here has finished (griddepcontrol.wait returns once the prerequisite grid has completed and its writes are visible), so no CTA
+// can see a slot's index move in the middle of its step.
+constexpr int SLOT_SCALARS = 3;
+
+__global__ void cfg_euler_slots_kernel(const float* __restrict__ eps, float* __restrict__ x, __half* __restrict__ unet_in, float* __restrict__ t_dev,
+                                       const int* __restrict__ state, const float* __restrict__ sig, const float* __restrict__ ts,
+                                       const float* __restrict__ scal, int S, int hw, int mode, int max_steps, unsigned long long fresh_mask) {
+  pdl_wait();
+  pdl_trigger();
+  const long long total = (long long)S * hw;
+  for (long long r = blockIdx.x * (long long)blockDim.x + threadIdx.x; r < total; r += (long long)gridDim.x * blockDim.x) {
+    const int p = (int)(r % hw);
+    const int s = (int)(r / hw);
+    const float* sg = sig + (long long)s * (max_steps + 1);
+    float sigma = 0.f, sigma_next, g = 0.f, ig = 0.f, init_sigma = 0.f;
+    if (eps == nullptr) {
+      if (!((fresh_mask >> s) & 1ull)) continue;
+      sigma_next = sg[0];
+      init_sigma = scal[s * SLOT_SCALARS + 2];
+      if (p == 0)
+        for (int br = 0; br < mode; ++br) t_dev[br * S + s] = ts[(long long)s * max_steps];
+    } else {
+      const int2 st = *(const int2*)(state + 2 * s);
+      if (st.x >= st.y) continue;
+      sigma = sg[st.x];
+      sigma_next = sg[st.x + 1];
+      g = scal[s * SLOT_SCALARS + 0];
+      ig = scal[s * SLOT_SCALARS + 1];
+    }
+    float4 e4[3] = {};
+    if (eps != nullptr) {
+#pragma unroll
+      for (int br = 0; br < 3; ++br)
+        if (br < mode) e4[br] = __ldg((const float4*)(eps + (((long long)(br * S + s)) * hw + p) * 4));
+    }
+    uint32_t o[4];
+#pragma unroll
+    for (int ch = 0; ch < 4; ++ch) {
+      const long long xi = ((long long)s * 4 + ch) * hw + p;
+      const float xv = x[xi];
+      const float xn = eps == nullptr ? xv * init_sigma
+                                      : cfg_euler_update([&](int br) { return (&e4[br].x)[ch]; }, xv, mode, g, ig, sigma, sigma_next);
+      x[xi] = xn;
+      o[ch] = __half_as_ushort(cfg_euler_input(xn, sigma_next));
+    }
+    const uint2 ov = make_uint2(o[0] | (o[1] << 16), o[2] | (o[3] << 16));
+    for (int br = 0; br < mode; ++br) *(uint2*)(unet_in + (((long long)(br * S + s)) * hw + p) * 8) = ov;
+  }
+}
+
+// one thread per slot: a live slot moves to its next step and, while one remains, its t_dev rows take that step's timestep
+__global__ void cfg_euler_slots_advance_kernel(float* __restrict__ t_dev, int* __restrict__ state, const float* __restrict__ ts, int S, int mode,
+                                               int max_steps) {
+  pdl_wait();                               // the combine launch has completed: nothing reads state[s][0] any more in this step
+  pdl_trigger();
+  const int s = threadIdx.x;
+  if (s >= S) return;
+  const int i = state[2 * s], n = state[2 * s + 1];
+  if (i >= n) return;
+  state[2 * s] = i + 1;
+  if (i + 1 < n)
+    for (int br = 0; br < mode; ++br) t_dev[br * S + s] = ts[(long long)s * max_steps + i + 1];
 }
 
 
@@ -583,6 +663,32 @@ extern "C" int seedx_cfg_euler_step(const float* eps, float* x, void* unet_in, i
                                                                                    guidance, image_guidance, sigma, sigma_next, init_sigma);
   count_launch();
   return check_cuda(cudaGetLastError(), "cfg_euler launch");
+}
+
+extern "C" int seedx_cfg_euler_slots(const float* eps, float* x, void* unet_in, float* t_dev, int32_t* state, const float* sigmas,
+                                     const float* timesteps, const float* scalars, int64_t slots, int64_t hw, int branches, int64_t max_steps,
+                                     uint64_t fresh_mask, void* stream) {
+  SEEDX_REQUIRE(branches == 2 || branches == 3, "seedx_cfg_euler_slots: branches must be 2 or 3 (got %d)", branches);
+  SEEDX_REQUIRE(x && unet_in && t_dev, "seedx_cfg_euler_slots: null x, unet_in or t_dev");
+  SEEDX_REQUIRE(state && sigmas && timesteps && scalars, "seedx_cfg_euler_slots: null slot state or table pointer");
+  SEEDX_REQUIRE(max_steps >= 1, "seedx_cfg_euler_slots: max_steps must be >= 1 (got %lld)", (long long)max_steps);
+  SEEDX_REQUIRE(slots >= 1 && slots <= 64 && hw >= 1, "seedx_cfg_euler_slots: slots=%lld hw=%lld (1 <= slots <= 64, hw >= 1)", (long long)slots,
+                (long long)hw);
+  SEEDX_REQUIRE((uintptr_t)unet_in % 16 == 0 && (uintptr_t)state % 8 == 0 && (!eps || (uintptr_t)eps % 16 == 0),
+                "seedx_cfg_euler_slots: eps and unet_in must be 16-byte aligned, state 8-byte aligned");
+  const uint64_t all = slots == 64 ? ~0ull : ((1ull << slots) - 1);
+  if (eps) SEEDX_REQUIRE(fresh_mask == 0, "seedx_cfg_euler_slots: fresh_mask only applies to the initialisation (eps == NULL)");
+  else SEEDX_REQUIRE(fresh_mask != 0 && (fresh_mask & ~all) == 0, "seedx_cfg_euler_slots: fresh_mask must name at least one of the %lld slots",
+                     (long long)slots);
+  cudaStream_t st = (cudaStream_t)stream;
+  launch_k(cfg_euler_slots_kernel, grid_for(slots * hw, 256), 256, 0, st, eps, x, (__half*)unet_in, t_dev, (const int*)state, sigmas, timesteps,
+           scalars, (int)slots, (int)hw, branches, (int)max_steps, (unsigned long long)fresh_mask);
+  count_launch();
+  if (int e = check_cuda(cudaGetLastError(), "cfg_euler_slots launch")) return e;
+  if (!eps) return 0;
+  launch_k(cfg_euler_slots_advance_kernel, 1, 64, 0, st, t_dev, (int*)state, timesteps, (int)slots, branches, (int)max_steps);
+  count_launch();
+  return check_cuda(cudaGetLastError(), "cfg_euler_slots_advance launch");
 }
 
 extern "C" int seedx_add_bcast_f16(const void* a, int a_dtype, const float* b, int64_t rows, int64_t cols, int64_t b_rows, void* out,

@@ -477,6 +477,29 @@ def cfg_euler_step(eps, x, unet_in, branches, guidance, image_guidance, sigma, s
     return x
 
 
+def cfg_euler_slots(eps, x, unet_in, t_dev, state, sigmas, timesteps, scalars, branches, fresh=None):
+    """seedx_cfg_euler_slots: one CFG + Euler step of every live slot (eps given), or the initialisation of the slots listed in `fresh`
+    (eps None).  x fp32 [S,4,h,w], unet_in fp16 [branches*S,h,w,8], t_dev fp32 [branches*S], state int32 [S,2] (step index, step count),
+    sigmas fp32 [S,max_steps+1], timesteps fp32 [S,max_steps], scalars fp32 [S,3] (guidance, image guidance, init_noise_sigma)."""
+    _require_cuda(eps, x, unet_in, t_dev, state, sigmas, timesteps, scalars)
+    assert x.dtype == torch.float32 and x.is_contiguous() and unet_in.dtype == torch.float16 and unet_in.is_contiguous()
+    S, c, h, w = x.shape
+    assert c == 4 and unet_in.shape == (branches * S, h, w, 8) and t_dev.dtype == torch.float32 and t_dev.numel() == branches * S
+    M = timesteps.shape[1]
+    assert state.dtype == torch.int32 and state.shape == (S, 2) and state.is_contiguous()
+    for t, shape in ((sigmas, (S, M + 1)), (timesteps, (S, M)), (scalars, (S, 3))):
+        assert t.dtype == torch.float32 and t.is_contiguous() and t.shape == shape
+    if eps is not None:
+        assert eps.dtype == torch.float32 and eps.is_contiguous() and eps.numel() == branches * S * h * w * 4
+    mask = 0
+    for s in fresh or ():
+        mask |= 1 << int(s)
+    check(lib().seedx_cfg_euler_slots(_ptr(eps), _ptr(x), _ptr(unet_in), _ptr(t_dev), _ptr(state), _ptr(sigmas), _ptr(timesteps), _ptr(scalars),
+                                      _i64(S), _i64(h * w), C.c_int(branches), _i64(M), C.c_uint64(mask), _stream()),
+          "seedx_cfg_euler_slots")
+    return x
+
+
 def gemv(W, x, out, *, rms_w=None, eps=1e-5, residual=None, gated=False, scale=None):
     """out[b] fp32 = epi(W[N,K] . (rmsnorm(x[b])*rms_w | x[b])); x fp32 [K] or [B,K] with B in {1,2,4,8} (weights streamed once).
     W fp16, or float8_e4m3fn with scale = fp32 [N] (weight row n = scale[n] * W[n]; seedx_gemv_fp8)."""
